@@ -1,4 +1,4 @@
-"""bagua_b200 — a Blackwell-native (sm_100a, NVLink 5 / NVSwitch) data-parallel training engine with the capabilities
+"""bagua_b200 — a Hopper-native (sm_90a, NVLink 4 / NVSwitch) data-parallel training engine with the capabilities
 and public API of BaguaSys/bagua (``import bagua_b200 as bagua`` or, unchanged user code, ``import bagua.torch_api as bagua``).
 
 Public surface mirrors ``bagua/torch_api/__init__.py:25-63`` of the reference."""

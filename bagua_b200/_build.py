@@ -1,8 +1,8 @@
-"""In-tree build of the native core (``bagua_b200/_C.so``) for sm_100a.
+"""In-tree build of the native core (``bagua_b200/_C.so``) for sm_90a (H100).
 
 The reference builds its Rust/C++ core for every ``sm_XX`` nvcc knows
 (rust/bagua-core/bagua-core-internal/build.rs:16-35).  This project targets exactly one
-architecture: ``-gencode arch=compute_100a,code=sm_100a``.  Sources are compiled with plain
+architecture: ``-gencode arch=compute_90a,code=sm_90a``.  Sources are compiled with plain
 ``nvcc``/``g++`` (no torch headers → seconds per file) and linked into one shared object that lives
 next to the python package, so it travels with the source tree.
 """
@@ -27,7 +27,7 @@ CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.environ.get("NVCC", str(Path(CUDA_HOME) / "bin" / "nvcc"))
 CXX = os.environ.get("CXX", "g++")
 
-GENCODE = ["-gencode", "arch=compute_100a,code=sm_100a"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-fvisibility=hidden", "-Wall", "-Wno-unused-function"]
 
@@ -105,7 +105,7 @@ def _tree_stamp() -> str:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every source under csrc/ for sm_100a and link ``bagua_b200/_C.so`` (incremental).
+    """Compile every source under csrc/ for sm_90a and link ``bagua_b200/_C.so`` (incremental).
 
     The object cache (``csrc/build``) does not travel with a snapshot of the tree, the library and its stamp do: when the
     stamp matches the sources nothing is compiled, so a GPU box that received a current ``_C.so`` starts immediately."""

@@ -2,7 +2,7 @@
 
 Reference: ``bagua/torch_api/bucket.py:18-366`` (API parity: padding/alignment, flatten, ``append_*_op``).
 
-B200-first: when the group has a :class:`~bagua_b200.parallel.symm.PeerEngine`, the flat storage of a bucket is a
+H100-first: when the group has a :class:`~bagua_b200.parallel.symm.PeerEngine`, the flat storage of a bucket is a
 slice of NVSwitch *symmetric memory* — the gradients (or weights) autograd/optimizers write are directly loadable
 by every peer GPU, so a bucket's op is a single fused kernel (no staging copy, no NCCL).  Without an engine
 (CPU/gloo, multi-node, ``BAGUA_ALLREDUCE_VARIANT=nccl``) the same ops run on ``torch.distributed``.

@@ -3,13 +3,13 @@
 Capability parity with ``bagua/torch_api/communication.py`` of the reference (init_process_group :446-548,
 new_group :206-273, from_torch_group :279-309, the 20 blocking collectives :573-1401, ReduceOp :64-75).
 
-B200-first design:
+H100-first design:
 
 * one process per GPU; ``torch.distributed`` (NCCL on GPUs, gloo on CPU) is the *plumbing*: rendezvous, object
   exchange, the cold user-facing primitives and the fallback for every op.  The reference is GPU/NCCL only
   (communication.py:540-546, :585); the gloo path lets the whole engine run and be tested without a GPU.
 * the *hot* paths (bucket allreduce, ByteGrad, decentralized averaging, MoE dispatch) do not go through this
-  file at all: they are sm_100a kernels over NVSwitch symmetric memory owned by :class:`PeerEngine`
+  file at all: they are sm_90a kernels over NVSwitch symmetric memory owned by :class:`PeerEngine`
   (``bagua_b200/parallel/symm.py``), reached through ``BaguaProcessGroup.peer_engine()``.
 * a communicator is (torch ProcessGroup, comm stream); blocking collectives keep the reference's stream
   protocol: current stream → event → comm stream runs the op → host waits for the comm stream.

@@ -3,7 +3,7 @@
 ``fuse_optimizer(opt)`` returns an optimizer with ``fuse_step()``.  Two engines sit behind it:
 
 * **kernel path** — for ``torch.optim.SGD / Adam / AdamW`` on CUDA the step of every parameter group is executed by the
-  sm_100a multi-tensor / flat kernels (``bagua_b200.ops.optim``): one launch per group instead of one per op per tensor.
+  sm_90a multi-tensor / flat kernels (``bagua_b200.ops.optim``): one launch per group instead of one per op per tensor.
 * **generic path** — for *any* other optimizer (and on CPU) the reference's idea is kept: tensors that are contiguous in
   memory simultaneously for weights, gradients and every state entry are viewed as ONE parameter, the optimizer's own
   ``step()`` runs on those few fused parameters, and the resulting state is sliced back (so it stays contiguous and fusable).

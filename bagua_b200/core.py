@@ -1,4 +1,4 @@
-"""Loader of the native core ``bagua_b200._C`` (C++ scheduler + sm_100a kernels).
+"""Loader of the native core ``bagua_b200._C`` (C++ scheduler + sm_90a kernels).
 
 On a box with a GPU the extension is mandatory — every hot op is a kernel in it and nothing silently falls back
 to eager PyTorch.  It is built in-tree on first import if missing (``bagua_b200/_build.py``).
@@ -46,7 +46,7 @@ def native():
         if _C is None:
             raise RuntimeError(
                 "bagua_b200 native core (_C.so) is not available: build it with `python -m bagua_b200._build` "
-                f"(nvcc, sm_100a). Import error: {_load_error!r}"
+                f"(nvcc, sm_90a). Import error: {_load_error!r}"
             )
         return _C
 

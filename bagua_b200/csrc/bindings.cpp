@@ -53,7 +53,7 @@ extern "C" __attribute__((visibility("default"))) void bagua_native_mark_ready(v
 }
 
 PYBIND11_MODULE(_C, m) {
-    m.doc() = "bagua_b200 native core (sm_100a)";
+    m.doc() = "bagua_b200 native core (sm_90a)";
     m.def("nhwc_api_ptr", [] { return reinterpret_cast<uint64_t>(bagua_nhwc_api()); });
     m.def("native_mark_ready_fn", [] { return reinterpret_cast<uint64_t>(&bagua_native_mark_ready); });
     m.def("backend_raw_ptr", [](Backend& b) { return reinterpret_cast<uint64_t>(&b); });
@@ -69,7 +69,7 @@ PYBIND11_MODULE(_C, m) {
     m.def("show_version", [] {
         int rt = 0;
         cudaRuntimeGetVersion(&rt);
-        return std::string("bagua_b200 native core; target sm_100a; cuda runtime ") + std::to_string(rt);
+        return std::string("bagua_b200 native core; target sm_90a; cuda runtime ") + std::to_string(rt);
     });
     m.def("launch_count", &launch_count);
     m.def("signal_pad_bytes", &PeerComm::signal_pad_bytes);

@@ -1,4 +1,4 @@
-// CTA-wide streaming reader on the TMA bulk-copy engine (sm_100a): global memory → ring of shared-memory stages via
+// CTA-wide streaming reader on the TMA bulk-copy engine (sm_90a): global memory → ring of shared-memory stages via
 // `cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes`, completion tracked by one mbarrier per stage.
 //
 // Why: the bandwidth a CTA can pull is (bytes in flight) / latency. A per-thread `ld.global` loop keeps at most a few 16-byte

@@ -42,7 +42,7 @@ int guarded(F&& f) {
 extern "C" {
 
 const char* bagua_last_error(void) { return g_last_error.c_str(); }
-const char* bagua_version(void) { return "bagua_b200 native core (sm_100a)"; }
+const char* bagua_version(void) { return "bagua_b200 native core (sm_90a)"; }
 
 BaguaTensorC* bagua_tensor_c_create(const char* name, uint64_t data_ptr, int64_t num_elements, int dtype, int device_id) {
     BaguaTensorC* out = nullptr;

@@ -30,7 +30,7 @@ inline size_t dtype_size(int dt) {
 // Reduction op codes — same numbering as the reference's ReduceOp (bagua/torch_api/communication.py:64-75).
 enum RedOp : int { SUM = 0, PRODUCT = 1, MIN = 2, MAX = 3, BOR = 7, BAND = 8, BXOR = 9, AVG = 10 };
 
-constexpr int kMaxPeers = 8;        // one NVSwitch domain (HGX B200 = 8 GPUs)
+constexpr int kMaxPeers = 8;        // one NVSwitch domain (HGX H100 = 8 GPUs)
 constexpr int kMaxCommBlocks = 256;  // upper bound on CTAs of any peer kernel (flag slots per block)
 constexpr int kFlagStride = kMaxPeers;
 // Behind the barrier flags every signal pad carries a small "vote" area: slot [s] is written by rank s (all of its CTAs write

@@ -1,6 +1,6 @@
 // Single-GPU bandwidth kernels: MinMaxUInt8 (de)compression, chunk reduce, async-average apply, axpby, cast.
-// Counterparts of the reference's scalar kernels (kernels/bagua_kernels.cu:196-690) written for HBM3e:
-// 16-byte accesses where alignment allows, grid sized to the 148 SMs, min/max fused into one pass
+// Counterparts of the reference's scalar kernels (kernels/bagua_kernels.cu:196-690) written for HBM3:
+// 16-byte accesses where alignment allows, grid sized to the 132 SMs of an H100, min/max fused into one pass
 // (the reference does 2 cub reductions per chunk from a host loop, bagua_kernels.cu:540-546).
 #include <stdexcept>
 #include <string>
@@ -13,7 +13,7 @@ using namespace dev;
 
 namespace {
 constexpr int kThreads = 512;
-inline int grid_for(size_t work_items, int per_thread = 4, int max_blocks = 148 * 8) {
+inline int grid_for(size_t work_items, int per_thread = 4, int max_blocks = 132 * 8) {
     size_t b = (work_items + static_cast<size_t>(kThreads) * per_thread - 1) / (static_cast<size_t>(kThreads) * per_thread);
     if (b < 1) b = 1;
     if (b > static_cast<size_t>(max_blocks)) b = max_blocks;
@@ -103,7 +103,7 @@ void launch_minmax_uint8_compress(const void* in, size_t numel, int dtype, int n
     const int count = target_chunk < 0 ? n_chunks : 1;
     auto* mm = reinterpret_cast<uint32_t*>(minmax_scratch);
     minmax_init_kernel<<<(2 * n_chunks + 255) / 256, 256, 0, stream>>>(mm, 2 * n_chunks);
-    dim3 grid(grid_for(chunk, 8, 148 * 4 / (count > 4 ? 4 : 1)), count);
+    dim3 grid(grid_for(chunk, 8, 132 * 4 / (count > 4 ? 4 : 1)), count);
     dispatch_float(dtype, [&](auto tag) {
         using T = decltype(tag);
         chunk_minmax_kernel<T><<<grid, kThreads, 0, stream>>>(static_cast<const T*>(in), chunk, first, mm);
@@ -117,7 +117,7 @@ void launch_minmax_uint8_decompress(const uint8_t* in, size_t numel, int dtype, 
     if (n_chunks <= 0 || numel % n_chunks) throw std::runtime_error("bagua: decompress needs numel divisible by n_chunks");
     const size_t chunk = numel / n_chunks;
     if (chunk == 0) return;
-    dim3 grid(grid_for(chunk, 8, 148 * 4 / (n_chunks > 4 ? 4 : 1)), n_chunks);
+    dim3 grid(grid_for(chunk, 8, 132 * 4 / (n_chunks > 4 ? 4 : 1)), n_chunks);
     dispatch_float(dtype, [&](auto tag) {
         using T = decltype(tag);
         chunk_dequantize_kernel<T><<<grid, kThreads, 0, stream>>>(in, chunk, minmax_uint8_chunk_bytes(chunk), static_cast<T*>(out));

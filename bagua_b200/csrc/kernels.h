@@ -1,4 +1,4 @@
-// Host-callable launchers of every CUDA kernel in bagua_b200 (implemented in *.cu, sm_100a).
+// Host-callable launchers of every CUDA kernel in bagua_b200 (implemented in *.cu, sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -89,7 +89,7 @@ struct BaguaNhwcApi {
 const BaguaNhwcApi* bagua_nhwc_api();
 }
 
-// ---- tcgen05 grouped GEMM (gemm_tcgen05.cu) ----------------------------------------------------------------------
+// ---- wgmma grouped GEMM (gemm_wgmma.cu) --------------------------------------------------------------------------
 // C[g] = act(A[g]·B[g]^T + bias[g]); A [G,M,K], B [G,N,K], C [G,M,N] bf16 (K-contiguous operands), bias fp32 [G,N] or null; act: 0 none, 1 GELU(tanh)
 bool grouped_gemm_supported(int M, int N, int K);
 void launch_grouped_gemm_tn(const void* A, const void* B, void* C, const float* bias, int G, int M, int N, int K, int act, cudaStream_t stream);

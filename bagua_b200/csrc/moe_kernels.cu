@@ -1,4 +1,4 @@
-// MoE expert-parallel token exchange as peer-memory kernels (sm_100a, NVLink 5 / NVSwitch).
+// MoE expert-parallel token exchange as peer-memory kernels (sm_90a, NVLink 4 / NVSwitch).
 //
 // The reference dispatches with a dense one-hot einsum (S*E*C*M MACs) followed by torch's NCCL all_to_all_single, and
 // combines with another all-to-all + einsum (bagua/torch_api/model_parallel/moe/sharded_moe.py:352-374). Here the

@@ -1,10 +1,10 @@
-// Fused optimizers for sm_100a.
+// Fused optimizers for sm_90a.
 //
 // The reference's "generic fused optimizer" is a pure-python storage-aliasing trick that still runs the stock
 // per-op torch kernels (bagua/torch_api/contrib/fuse/optimizer.py:318-341; several passes over HBM per step).
 // Here the whole update of a flat arena — grad unscale, weight decay, momentum / Adam moments, fp32 master
 // update, cast of the new weights to the model dtype and zeroing of the gradient — is ONE pass with 16-byte
-// accesses, i.e. the HBM3e floor for an optimizer step. A chunked multi-tensor variant covers parameters that
+// accesses, i.e. the HBM3 floor for an optimizer step. A chunked multi-tensor variant covers parameters that
 // are not contiguous.
 #include <stdexcept>
 #include <string>
@@ -67,7 +67,7 @@ __device__ __forceinline__ void adam_update(float& w, float g, float& m, float& 
 
 inline int flat_grid(size_t numel) {
     size_t b = (numel + static_cast<size_t>(kThreads) * kVec - 1) / (static_cast<size_t>(kThreads) * kVec);
-    const size_t cap = 148 * 4;  // 4 resident CTAs of 512 threads per SM
+    const size_t cap = 132 * 4;  // 4 resident CTAs of 512 threads per SM (H100: 132 SMs)
     if (b > cap) b = cap;
     if (b < 1) b = 1;
     return static_cast<int>(b);

@@ -1,9 +1,8 @@
 // Fused NHWC (channels_last) epilogues for convolutional blocks: bias + ReLU (+ 2x2/2 max-pool) forward and backward.
 //
 // In eager PyTorch a conv block is conv → bias add → ReLU → max-pool, each a full pass over the activation tensor, and
-// the backward adds a ReLU mask pass, a (slow, strided) bias-gradient reduction and a generic max-pool backward. On B200
-// these bandwidth passes cost more than the tensor-core convolutions themselves (VGG16, bs 32: ≈4.5 ms of a 7.6 ms step,
-// profiles/vgg16_n1_torch_profiler.txt). Here every block epilogue is ONE pass with 16-byte accesses:
+// the backward adds a ReLU mask pass, a (slow, strided) bias-gradient reduction and a generic max-pool backward. These
+// bandwidth passes can cost more than the tensor-core convolutions themselves. Here every block epilogue is ONE pass with 16-byte accesses:
 //   fwd : y = relu(conv_out + bias)                       (in place)          | out, idx = maxpool2(relu(conv_out + bias))
 //   bwd : g' = g * (y > 0);  bias_grad += Σ g'                               | g_in = scatter(g * (out > 0), idx);  bias_grad += Σ
 // The convolution itself stays a library call (cuDNN); it is run without bias so cuDNN skips its own bias-grad reduction.
@@ -207,7 +206,7 @@ void check_c(int C) {
 }
 int grid_for(size_t items, int multiple_of = 1) {
     size_t b = (items + kThreads - 1) / kThreads;
-    const size_t cap = 148 * 8;
+    const size_t cap = 132 * 8;
     if (b > cap) b = cap;
     if (b < 1) b = 1;
     if (multiple_of > 1) b = (b + multiple_of - 1) / multiple_of * multiple_of;

@@ -1,6 +1,6 @@
-// Device-side building blocks for kernels that talk to other GPUs over NVLink 5 / NVSwitch:
+// Device-side building blocks for kernels that talk to other GPUs over NVLink 4 / NVSwitch:
 // system-scope flags, an epoch barrier over symmetric signal pads, 16-byte peer loads/stores and the
-// NVLS multimem instructions. sm_100a only.
+// NVLS multimem instructions. sm_90a only.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

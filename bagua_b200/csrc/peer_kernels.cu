@@ -1,4 +1,4 @@
-// Fused collective kernels over NVLink 5 / NVSwitch symmetric memory (sm_100a).
+// Fused collective kernels over NVLink 4 / NVSwitch symmetric memory (sm_90a).
 //
 // These replace the reference's "kernel + separate NCCL call" sequences
 // (rust/bagua-core/bagua-core-internal/src/comm_ops/*.rs, communicators/mod.rs:1121-1153): the reduction,

@@ -72,8 +72,8 @@ __device__ __forceinline__ uint8_t quantize(float x, const QuantParams& q) {
     return f32_to_u8_sat(__fsub_rn(level, q.lower));
 }
 // x' = (q + lower) / scale, evaluated as a multiplication by the chunk's reciprocal: an IEEE fp32 division is ~10 issue slots per
-// ELEMENT (MUFU.RCP + Newton steps + FCHK + slow-path call) and made up 39 % of the SASS of bytegrad_kernel<bf16, 8>, a kernel that ncu
-// shows to be instruction-issue bound (profiles/ncu_summary.md); the product differs from the quotient by at most one fp32 ulp, far below
+// ELEMENT (MUFU.RCP + Newton steps + FCHK + slow-path call) and made up 39 % of the SASS of bytegrad_kernel<bf16, 8>, a kernel that Nsight
+// Compute showed to be instruction-issue bound; the product differs from the quotient by at most one fp32 ulp, far below
 // a quantisation level, and every rank decodes with the same code, so replicas stay bit-identical. -DBAGUA_DEQUANT_IEEE_DIV restores the
 // division (bit-exact with the reference's formula, bagua_kernels.cu:456-501).
 __device__ __forceinline__ float dequantize(uint8_t v, const QuantParams& q) {

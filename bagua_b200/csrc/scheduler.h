@@ -4,7 +4,7 @@
 // ordered buckets, strictly-in-order scheduling, one background comm worker per backend, a watchdog,
 // duplicate detection at registration, waitable completion.
 //
-// B200-first differences:
+// H100-first differences:
 //  * the worker never host-synchronises a stream (the reference blocks the worker per bucket with
 //    cudaStreamSynchronize, datatypes/mod.rs:1110-1115). Ops are *launched* on the comm stream, a pooled
 //    event is recorded behind them, and wait_pending_comm_ops() makes the consumer stream wait on that

@@ -28,7 +28,7 @@ def gpt2_medium_moe8_config() -> GPT2MoEConfig:
 
 
 class ExpertMLP(nn.Module):
-    grouped_gemm_compatible = True  # fc2(gelu_tanh(fc1(x))): Experts runs all local experts as one tcgen05 grouped GEMM
+    grouped_gemm_compatible = True  # fc2(gelu_tanh(fc1(x))): Experts runs all local experts as one wgmma grouped GEMM
 
     def __init__(self, d):
         super().__init__()

@@ -1,4 +1,4 @@
-"""Grouped linear layers on the hand-written tcgen05/TMEM/TMA GEMM (csrc/gemm_tcgen05.cu).
+"""Grouped linear layers on the hand-written wgmma/TMA GEMM (csrc/gemm_wgmma.cu).
 
 ``grouped_linear(x[G,M,K], w[G,N,K], bias[G,N]) -> [G,M,N]`` computes ``x @ w^T + bias`` per group (per local expert).
 Forward and both backward GEMMs run on the same TN kernel (operands are brought into K-contiguous form with a transpose
@@ -17,12 +17,12 @@ __all__ = ["grouped_linear", "grouped_gemm_tn", "tcgen05_supported"]
 
 
 def tcgen05_supported(x: torch.Tensor, M: int, N: int, K: int) -> bool:
-    """Whether the tcgen05 grouped GEMM handles this problem: bf16 CUDA operands, ``M % 128 == 0``, ``N % 128 == 0``, ``K % 64 == 0``."""
+    """Whether the wgmma grouped GEMM handles this problem (the name is historical): bf16 CUDA operands, ``M % 128 == 0``, ``N % 128 == 0``, ``K % 64 == 0``."""
     return x.is_cuda and x.dtype == torch.bfloat16 and native().grouped_gemm_supported(M, N, K)
 
 
 def grouped_gemm_tn(a: torch.Tensor, b: torch.Tensor, bias: Optional[torch.Tensor] = None, act: str = "none") -> torch.Tensor:
-    """``out[g] = act(a[g] @ b[g]^T + bias[g])`` with a [G,M,K], b [G,N,K] contiguous bf16 CUDA tensors (tcgen05 kernel)."""
+    """``out[g] = act(a[g] @ b[g]^T + bias[g])`` with a [G,M,K], b [G,N,K] contiguous bf16 CUDA tensors (wgmma kernel)."""
     G, M, K = a.shape
     N = b.shape[1]
     assert b.shape[0] == G and b.shape[2] == K and a.is_contiguous() and b.is_contiguous()

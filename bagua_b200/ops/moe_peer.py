@@ -42,7 +42,7 @@ class MoEPeerContext:
     def _buf(self, nbytes: int, which: int, key=None):
         """Symmetric buffer for an exchange.  ``key is None``: the pair shared by every call site of this size (results must be
         copied out before the next exchange).  With a ``key`` (one per MoE layer and direction) the call site OWNS its buffer —
-        16 MiB per layer for GPT-2-medium MoE-8, nothing next to 180 GB — so the received rows are used in place: no ``clone``
+        16 MiB per layer for GPT-2-medium MoE-8, nothing next to 80 GB — so the received rows are used in place: no ``clone``
         behind the scatter.  Reuse is safe across iterations: a layer's next scatter opens with a cross-GPU barrier that every rank
         reaches only after (stream order) it has finished the previous iteration's backward, the last reader of the buffer."""
         pair = self._buffers.get((nbytes, key))
@@ -93,7 +93,7 @@ class MoEPeerContext:
     def linear_push_gather(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], expert_idx, slot_idx, weights: torch.Tensor, S: int,
                            C: int) -> Tuple[torch.Tensor, torch.Tensor]:
         """``combine(linear(x))`` with the all-to-all inside the GEMM: x [E_local, world*C, K] (rows ordered [source rank][slot]),
-        w [E_local, N, K].  The tcgen05 GEMM's epilogue stores every 128-row tile straight into the symmetric buffer of the
+        w [E_local, N, K].  The wgmma GEMM's epilogue stores every 128-row tile straight into the symmetric buffer of the
         rank the tokens came from; the local-layout gather (which opens with the peer barrier) then forms
         out[s] = Σ_k weights[s,k] · row.  Returns (out [S, N], picked [S, k, N])."""
         E_local, _, Kdim = x.shape

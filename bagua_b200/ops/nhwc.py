@@ -33,6 +33,13 @@ def _finish_in_kernel() -> bool:
     return os.environ.get("BAGUA_NHWC_FINALIZE", "0") == "1"
 
 
+def _deterministic() -> bool:
+    """Under ``torch.use_deterministic_algorithms(True)`` the bias gradient is torch's (fixed-order) sum of the masked gradient the
+    kernel writes, not the kernel's own atomic reduction, whose summation order varies from run to run; the rest of the backward
+    is the same kernel."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
 def _workspace(device: torch.device, stream: int) -> torch.Tensor:
     """Zeroed fp32[2048] sums + one uint32 ticket, per (device, stream): kernels on one stream run back to back and each one
     hands the buffer back zeroed, so it is allocated and cleared exactly once."""
@@ -60,7 +67,7 @@ class _BiasReLU(torch.autograd.Function):
         N, C, H, W = y.shape
         g = g.contiguous(memory_format=torch.channels_last)
         gout = torch.empty_like(g, memory_format=torch.channels_last)
-        if _finish_in_kernel():
+        if _finish_in_kernel() and not _deterministic():
             stream = _stream()
             ws = _workspace(y.device, stream)
             bias_grad = torch.empty(C, dtype=ctx.bias_dtype, device=y.device)
@@ -69,6 +76,8 @@ class _BiasReLU(torch.autograd.Function):
             return gout, bias_grad
         bg = torch.zeros(C, dtype=torch.float32, device=y.device)
         native().bias_relu_nhwc_bwd(g.data_ptr(), y.data_ptr(), gout.data_ptr(), bg.data_ptr(), N * H * W, C, dtype_code(y.dtype), _stream())
+        if _deterministic():
+            bg = torch.sum(gout, dim=(0, 2, 3), dtype=torch.float32)
         return gout, bg.to(ctx.bias_dtype)
 
 
@@ -90,7 +99,7 @@ class _BiasReLUMaxPool2(torch.autograd.Function):
         N, C, H, W = ctx.in_shape
         g = g.contiguous(memory_format=torch.channels_last)
         gin = torch.empty((N, C, H, W), dtype=out.dtype, device=out.device, memory_format=torch.channels_last)
-        if _finish_in_kernel():
+        if _finish_in_kernel() and not _deterministic():
             stream = _stream()
             ws = _workspace(out.device, stream)
             bias_grad = torch.empty(C, dtype=ctx.bias_dtype, device=out.device)
@@ -100,6 +109,8 @@ class _BiasReLUMaxPool2(torch.autograd.Function):
         bg = torch.zeros(C, dtype=torch.float32, device=out.device)
         native().bias_relu_pool_nhwc_bwd(g.data_ptr(), out.data_ptr(), idx.data_ptr(), gin.data_ptr(), bg.data_ptr(), N, H, W, C, dtype_code(out.dtype),
                                          _stream())
+        if _deterministic():   # gin holds every masked gradient exactly once (zeros elsewhere): same sum as the kernel's
+            bg = torch.sum(gin, dim=(0, 2, 3), dtype=torch.float32)
         return gin, bg.to(ctx.bias_dtype)
 
 
@@ -107,7 +118,10 @@ _native_fns = [False]
 
 
 def _native_functions():
-    """C++ autograd Functions of the optional torch extension (opt-in ``BAGUA_NATIVE_NHWC=1``), or ``None``."""
+    """C++ autograd Functions of the optional torch extension (opt-in ``BAGUA_NATIVE_NHWC=1``), or ``None`` (also in deterministic
+    mode, which only the Python Functions implement)."""
+    if _deterministic():
+        return None
     if _native_fns[0] is False:
         ext = None
         if os.environ.get("BAGUA_NATIVE_NHWC", "0") == "1":

@@ -1,4 +1,4 @@
-"""Fused optimizers on the sm_100a multi-tensor / flat kernels (csrc/multi_tensor.cu).
+"""Fused optimizers on the sm_90a multi-tensor / flat kernels (csrc/multi_tensor.cu).
 
 Reference: ``bagua/torch_api/contrib/fuse/optimizer.py`` fuses by *aliasing* contiguous tensors and then runs the stock
 torch ``step()`` (several element-wise kernels, several passes over HBM).  Here a step over a bucket-flattened model is
@@ -24,7 +24,7 @@ def _stream() -> int:
 
 
 def _kernels_apply(params) -> bool:
-    """The sm_100a kernels handle CUDA tensors; everything else takes the plain torch update (also the hook the CPU tests use to
+    """The sm_90a kernels handle CUDA tensors; everything else takes the plain torch update (also the hook the CPU tests use to
     drive the kernel call sites with a host double)."""
     return params[0].device.type == "cuda"
 

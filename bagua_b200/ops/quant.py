@@ -88,7 +88,7 @@ def torch_decompress(buf: torch.Tensor, numel: int, n_chunks: int, dtype: torch.
 
 # ---- kernel wrappers ------------------------------------------------------------------------------------------
 def compress(x: torch.Tensor, n_chunks: int = 1, target_chunk: int = -1, out: torch.Tensor | None = None) -> torch.Tensor:
-    """MinMaxUInt8-compress ``x`` (sm_100a kernel on CUDA tensors, torch elsewhere)."""
+    """MinMaxUInt8-compress ``x`` (sm_90a kernel on CUDA tensors, torch elsewhere)."""
     assert x.is_contiguous() and x.numel() % n_chunks == 0
     if x.device.type != "cuda":
         full = torch_compress(x, n_chunks)

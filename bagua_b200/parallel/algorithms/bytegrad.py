@@ -15,8 +15,7 @@ def bytegrad_min_bucket_bytes(tensors) -> int:
     """Lower bound on a ByteGrad bucket on GPUs (``BAGUA_BYTEGRAD_MIN_BUCKET_BYTES``, default 32 MiB; 0 on the host).  Every quantised
     exchange — the fused kernel as well as the 7-step torch.distributed pipeline — has a fixed cost per bucket (four grid-wide and two
     cross-GPU rendezvous in the kernel; 2·P+7 launches and two collectives in the pipeline) that does not shrink with the bucket, while
-    NVSwitch moves 10 MiB in microseconds.  Measured on BERT-large, 1 GPU (profiles/r2/bytegrad_tuning_n1.md): 48 buckets of 10 MiB and
-    17 of 32 MiB train at the same speed with 64 CTAs (304 samples/s); the merge pays where the rendezvous cross GPUs."""
+    NVSwitch moves 10 MiB in microseconds, so fewer, larger buckets pay where the rendezvous cross GPUs."""
     import os
 
     try:

@@ -369,9 +369,8 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         momentum = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
         # NVLS whenever the fabric offers it (the variant validated on 2 and 8 GPUs); peer ld/st two-shot otherwise
         use_mc = bool(wslice.has_multicast and bucket._slice.has_multicast and eng.has_multicast)
-        # with 2 ranks the in-switch reduction buys nothing (each GPU pulls half the bucket either way) and the peer ld/st kernel
-        # is the faster one on the plain allreduce (profiles/allreduce_n2.json: two-shot 654 vs multimem 402 GB/s): same policy
-        # as PeerEngine.choose_variant. BAGUA_FUSED_MULTIMEM=0/1 forces either flavour.
+        # with 2 ranks the in-switch reduction buys nothing (each GPU pulls half the bucket either way), so the peer ld/st
+        # kernel is used: same policy as PeerEngine.choose_variant. BAGUA_FUSED_MULTIMEM=0/1 forces either flavour.
         force = os.environ.get("BAGUA_FUSED_MULTIMEM", "auto")
         if force == "0" or (force != "1" and n <= 2):
             use_mc = False

@@ -3,7 +3,7 @@
 Capability parity with ``bagua/torch_api/data_parallel/bagua_distributed.py`` (hooks :93-148, param build :155-212,
 state broadcast :229-323, autotune :325-391, hook registration :417-481, bucket reset :483-496).
 
-B200-first changes of the hot path:
+H100-first changes of the hot path:
 
 * one forward-pre hook and one *post-accumulate-grad* hook per parameter whose closure is built once per
   (re)initialisation — the reference rebuilds the algorithm's hook closure for every gradient of every iteration

@@ -18,7 +18,7 @@ class Experts(torch.nn.Module):
 
     def _grouped_mlp(self):
         """(fc1, fc2, activation) lists when every local expert is a 2-layer MLP ``fc2(act(fc1(x)))`` — the shape the
-        tcgen05 grouped GEMM accelerates; ``None`` otherwise."""
+        wgmma grouped GEMM accelerates; ``None`` otherwise."""
         cached = getattr(self, "_grouped_cache", None)
         if cached is not None:
             return cached or None

@@ -4,7 +4,7 @@
 Semantics kept: fp32 gate, capacity = ceil(tokens/experts·factor) (≥ ``min_capacity`` for top-1), random token selection
 under overflow for top-1, Gumbel-max second expert for top-2, the auxiliary load-balancing loss, ``exp_counts`` (kept on the device unless ``BAGUA_MOE_EXP_COUNTS_ON_CPU=1``).
 
-B200-first formulation: gating produces *indices* — for every token and choice k: expert id, slot in that expert's
+H100-first formulation: gating produces *indices* — for every token and choice k: expert id, slot in that expert's
 capacity buffer (or dropped) and combine weight — instead of the reference's dense one-hot ``[S, E, C]`` tensors, whose
 ``einsum("sec,sm->ecm")`` dispatch costs S·E·C·M MACs (sharded_moe.py:352-354).  Dispatch is then a row scatter and combine
 a weighted row gather; on NVSwitch both are kernels that store/load token rows directly in the destination expert's

@@ -1,8 +1,8 @@
 """NVSwitch symmetric-memory engine: the per-group state behind every fused collective kernel.
 
 There is no counterpart in the reference — its communicators are NCCL handles
-(rust/bagua-core/bagua-core-internal/src/communicators/mod.rs:26-73).  On an HGX B200 every GPU reaches every
-peer at full NVLink 5 bandwidth through NVSwitch, so a group's "communicator" here is:
+(rust/bagua-core/bagua-core-internal/src/communicators/mod.rs:26-73).  On an HGX H100 every GPU reaches every
+peer at full NVLink 4 bandwidth through NVSwitch, so a group's "communicator" here is:
 
 * symmetric device memory: identical allocations on every rank, each mapped into every peer's address space
   (+ an NVLS multicast alias when the fabric offers it).  Allocation/handle exchange is bootstrapped with
@@ -248,8 +248,8 @@ class PeerEngine:
             return row["variant"]
         if nbytes <= ONE_SHOT_SLOT // 2:
             return "one_shot"
-        # measured (profiles/allreduce_n*.json): with 2 ranks the peer-load two-shot kernel beats the in-switch reduction
-        # (654 vs 402 GB/s at 256 MiB); from 4 ranks on multimem moves ~N/2 x fewer bytes over each GPU's links
+        # with 2 ranks each GPU pulls half the bucket either way, so the in-switch reduction saves nothing and the peer-load two-shot
+        # kernel is used; from 4 ranks on multimem moves ~N/2 x fewer bytes over each GPU's links
         if self.world <= 2:
             return "two_shot"
         return "multimem" if self.has_multicast else "two_shot"
@@ -268,7 +268,7 @@ class PeerEngine:
             if variant == "one_shot":
                 blocks = max(1, min(8, vecs // 512))
             elif variant == "multimem":
-                blocks = max(1, min(8, vecs // (self.world * 2048)))  # 8 CTAs saturate NVLS (profiles/allreduce_n8.json)
+                blocks = max(1, min(8, vecs // (self.world * 2048)))  # 8 CTAs of 512 threads keep enough NVLS requests in flight
             else:
                 blocks = max(1, min(32, vecs // (self.world * 2048)))
         return C.LaunchCfg(int(min(blocks, C.MAX_COMM_BLOCKS)), 512)

@@ -4,7 +4,7 @@ The fused collective kernels (``csrc/peer_kernels.cu``, ``csrc/bytegrad_kernels.
 pointers: ``PeerCtx.flags[p]`` (signal pads), ``PeerBuf.ptr[p]`` (one buffer per rank) and their own ``rank``.  Nothing in
 them requires the P buffers to live on P different GPUs — so a *virtual world* gives every rank its own signal pad,
 buffers and CUDA stream on the same device and launches the P kernels back to back on the P streams.  They become
-co-resident (P × grid ≤ what the 148 SMs hold), meet at the same epoch barriers and exchange data through the same
+co-resident (P × grid ≤ what the 132 SMs of an H100 hold), meet at the same epoch barriers and exchange data through the same
 loads/stores as over NVLink; only the wires are missing.  That makes every P = 2…8 code path (slice arithmetic, rotation of
 the peer order, barrier protocol, parity double-buffering, quantised in/out boxes, MoE row addressing) checkable against
 fp32 oracles on a single-GPU box — which is what the CI box has (the reference can only test its collectives with ≥ 2

@@ -26,7 +26,7 @@ def _lib_state() -> Dict[str, dict]:
         stamp_ok = _build.STAMP.exists() and _build.STAMP.read_text().strip() == _build._tree_stamp()
     except Exception as e:  # noqa: BLE001
         stamp_ok = f"unknown ({e})"
-    for name, path, current in (("_C.so (native core, sm_100a kernels)", _build.TARGET, stamp_ok),
+    for name, path, current in (("_C.so (native core, sm_90a kernels)", _build.TARGET, stamp_ok),
                                 ("libnccl-net-bagua.so (NCCL net plugin)", _build.NET_TARGET, None),
                                 ("_C_torch.so (optional C++ autograd hooks)", _build.PKG_DIR / "_C_torch.so", None)):
         out[name] = {"path": str(path), "present": path.exists(), "bytes": path.stat().st_size if path.exists() else 0}
@@ -66,8 +66,8 @@ def _gpus() -> dict:
         devs.append({"index": i, "name": p.name, "sm": f"{p.major}.{p.minor}", "sms": p.multi_processor_count, "memory_GiB": round(p.total_memory / 2 ** 30, 1)})
     peer = [[(i == j) or bool(torch.cuda.can_device_access_peer(i, j)) for j in range(n)] for i in range(n)]
     info = {"count": n, "devices": devs, "peer_access_all_pairs": all(all(r) for r in peer)}
-    if any(d["sm"] != "10.0" for d in devs):
-        info["warning"] = "the kernels are compiled for sm_100a only (B200); other architectures cannot load them"
+    if any(d["sm"] != "9.0" for d in devs):
+        info["warning"] = "the kernels are compiled for sm_90a only (H100); other architectures cannot load them"
     try:
         import torch.distributed._symmetric_memory as symm  # noqa: F401
 
@@ -169,7 +169,7 @@ def _self_test(peer_kernels: bool = False) -> List[dict]:
             assert torch.allclose(p, torch.full_like(p, 0.95))
             return "flat_sgd kernel"
 
-        check("fused optimizer kernel (sm_100a)", fused_step)
+        check("fused optimizer kernel (sm_90a)", fused_step)
         if peer_kernels:
             def virtual_world():
                 """A 4-rank all-reduce, a fused allreduce+SGD step and a ByteGrad exchange among VIRTUAL ranks on this one GPU
@@ -207,7 +207,7 @@ def main(argv=None) -> int:
     args = ap.parse_args(argv)
     report = {"libraries": _lib_state(), "versions": _versions(), "gpus": _gpus(), "environment": _environment()}
     report["self_test"] = [] if args.no_self_test else _self_test(peer_kernels=args.kernels)
-    ok = all(r["ok"] for r in report["self_test"]) and report["libraries"]["_C.so (native core, sm_100a kernels)"]["present"]
+    ok = all(r["ok"] for r in report["self_test"]) and report["libraries"]["_C.so (native core, sm_90a kernels)"]["present"]
     report["ok"] = bool(ok)
     if args.json:
         print(json.dumps(report, indent=1, default=str))

@@ -1,7 +1,7 @@
 """Whole-step CUDA graph capture for launch-bound training loops.
 
-The VGG16 step on one B200 issues ≈ 120 kernels in 4.3 ms; the host needs ≈ 3.9 ms to launch them (profiles/
-vgg16_n1_torch_profiler.txt), so any extra host work — data loading, logging, a slower CPU — shows up as idle GPU time.
+The VGG16 step issues ≈ 120 kernels and the host needs about as long to launch them as the GPU needs to run them, so any
+extra host work — data loading, logging, a slower CPU — shows up as idle GPU time.
 :class:`GraphedTrainStep` records one complete step (zero_grad → forward → loss → backward → optimizer) into a
 ``torch.cuda.CUDAGraph`` and replays it with a single launch; new inputs are copied into the static input tensors first.
 

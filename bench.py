@@ -2,8 +2,7 @@
 """Headline benchmark (BASELINE.json): VGG16 images/s (GradientAllReduce) AND BERT-large samples/s (ByteGrad), bf16, synthetic
 data of the named shapes, random-init weights, device-timed (CUDA events), max over ranks.
 
-Contract (task statement): ``python bench.py --gpus N --steps K --warmup W`` (launched through torchrun for N > 1) prints ONE
-JSON line from rank 0.  The top-level ``metric`` / ``value`` / ``e2e`` / … describe the VGG16 workload — the reference's own
+``python bench.py --gpus N --steps K --warmup W`` (launched through torchrun for N > 1) prints ONE JSON line from rank 0.  The top-level ``metric`` / ``value`` / ``e2e`` / … describe the VGG16 workload — the reference's own
 synthetic benchmark shape (examples/benchmark/synthetic_benchmark.py: bs 32/GPU, SGD, cross-entropy, fixed random batch) — and
 the ``bert_large_bytegrad`` block carries the same fields for the second half of the metric: BERT-large question answering on
 SQuAD-shaped batches (seq 384, bs 6/GPU as examples/squad/README.md:19-28) with the ByteGrad algorithm and AdamW.
@@ -12,7 +11,7 @@ Arms (``--impl``):
   ours           the framework as a user gets it: fused NVSwitch bucket kernels, fused optimizers.
   nccl_baseline  SAME models / optimizers / bucketing / scheduler with ``BAGUA_ALLREDUCE_VARIANT=nccl``: one NCCL all-reduce per
                  bucket, ByteGrad as the reference's 7-step compress → alltoall → … pipeline on torch.distributed — the re-expression
-                 of the reference's schedule that SURVEY §6 prescribes as the same-box baseline.  Context, never the driver's arm.
+                 of the reference's schedule that SURVEY §6 prescribes as the same-box baseline.  Context only.
   ddp            stock PyTorch: ``DistributedDataParallel`` + ``torch.optim`` + eager modules (no bagua_b200 kernel). Context.
   reference      the unmodified reference from ``baseline/_ref``; it cannot be installed offline in this image (Rust core: cargo,
                  setuptools_rust, mpicxx and a downloaded NCCL are all missing, DESIGN.md §3), so the arm reports itself unavailable.
@@ -24,6 +23,12 @@ they do at N = 8 — the scaling base is not flattered by a cheaper single-GPU c
 After each workload's timed regions six more steps run with the scheduler's per-bucket timeline on; the summary (``comm_timeline``:
 communication left exposed after backward, the bucket that finishes last, device time per bucket) explains the step time, it is
 not part of any timed region.  A failure of the second workload is reported in its block and does not take the first one's line with it.
+
+``--dump-outputs DIR`` writes, after the timed region of each workload, what its last timed step computed as float32 ``.npy``
+files: ``<workload>_loss.npy`` (the loss the step returned) and ``<workload>_params_sample.npy`` (the updated weights at a fixed,
+seeded sample of 2^20 positions of the parameters in model order).  Inputs and initial weights come from fixed seeds, so two runs
+or two builds with the same arguments can be compared output for output.  Such a run uses deterministic algorithms throughout
+(see main()) and is therefore slower than the plain throughput run.
 
 ``--selftest-cpu`` runs the same code end to end on the host with tiny shapes for the test-suite (marked ``selftest``).
 """
@@ -61,6 +66,7 @@ def parse():
                    help="fold the SGD update into the allreduce kernel (sharded optimizer state); default: on whenever the group has a peer engine")
     p.add_argument("--no-fused-shard", dest="fused_shard", action="store_false")
     p.add_argument("--cuda-graph", action="store_true", help="experimental: replay the whole VGG16 step from a CUDA graph (utils.graph.GraphedTrainStep)")
+    p.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed step's loss and a seeded sample of the updated weights as .npy files")
     p.add_argument("--selftest-cpu", action="store_true", help=argparse.SUPPRESS)
     p.add_argument("--image-size", type=int, default=224, help=argparse.SUPPRESS)
     return p.parse_args()
@@ -252,8 +258,27 @@ def launch_counter(c):
     return native().launch_count  # every kernel of this library counts itself (csrc/common.h: count_launch)
 
 
-def measure(c, name, train_step, dev_batch, host_batches, to_model_format, per_step_items, unit, finish=None):
-    """Warm-up, device-timed region, e2e region (pinned host batches → prefetcher → step → loss read-back)."""
+DUMP_SAMPLE = 1 << 20   # weights per workload in --dump-outputs (4 MB of float32)
+
+
+def sample_params(torch, params, n=DUMP_SAMPLE, seed=20240601):
+    """float32 values of the parameters (flattened and concatenated in model order) at ``n`` positions drawn from a fixed seed."""
+    params = list(params)
+    sizes = [p.numel() for p in params]
+    total = sum(sizes)
+    pos = torch.randint(0, total, (min(n, total),), generator=torch.Generator().manual_seed(seed)).sort().values
+    out, off = [], 0
+    for p, k in zip(params, sizes):
+        lo, hi = torch.searchsorted(pos, off), torch.searchsorted(pos, off + k)
+        if hi > lo:
+            out.append(p.detach().reshape(-1)[(pos[lo:hi] - off).to(p.device)].float().cpu())
+        off += k
+    return torch.cat(out)
+
+
+def measure(c, name, train_step, dev_batch, host_batches, to_model_format, per_step_items, unit, finish=None, params=None):
+    """Warm-up, device-timed region, e2e region (pinned host batches → prefetcher → step → loss read-back).  With
+    ``--dump-outputs`` the loss and a weight sample of the last timed step are kept in ``c.dumps`` before anything else runs."""
     torch = c.torch
     args = c.args
     from bagua_b200.utils.data import DevicePrefetcher, LossReader
@@ -294,6 +319,9 @@ def measure(c, name, train_step, dev_batch, host_batches, to_model_format, per_s
     loss_val = float(holder["loss"].detach().float().item())     # the loss of the last timed step, read after the timed region
     if loss_val != loss_val or loss_val in (float("inf"), float("-inf")):
         raise SystemExit(f"{name}: non-finite loss {loss_val} after the timed region — the number would be a throughput of nothing")
+    if args.dump_outputs and params is not None:
+        c.dumps[f"{name}_loss"] = holder["loss"].detach().float().reshape(1).cpu().numpy()
+        c.dumps[f"{name}_params_sample"] = sample_params(torch, params()).numpy()
     value = per_step_items * c.world * args.steps / (ms / 1e3)
     e2e = None
     if not args.no_e2e:
@@ -521,14 +549,14 @@ def run_cnn(c, model_name):
         for i in range(n):
             yield x_host[i % n_host], y_host[i % n_host]
 
-    res = measure(c, model_name, step_fn, (x_dev, y_dev), host_batches, to_model_format, bs, "images/s", finish)
+    res = measure(c, model_name, step_fn, (x_dev, y_dev), host_batches, to_model_format, bs, "images/s", finish, params=model.parameters)
     if args.impl != "ddp" and not args.cuda_graph:
         res["comm_timeline"] = timeline_probe(c, model, step_fn, (x_dev, y_dev), finish)
     algo = "GradientAllReduce"
     res["metric"] = f"{model_name} synthetic-ImageNet training throughput ({algo})"
     res["config"] = dict(cfg, model=model_name, global_batch=bs * world, per_gpu_batch=bs, image=f"3x{img}x{img}", parallelism=f"dp{world}",
                          algorithm=algo, lr=lr, momentum=args.momentum, cuda_graph=bool(args.cuda_graph),
-                         l2_policy="working set (276 MB bf16 weights + activations) far exceeds the 126 MB L2; no explicit flush")
+                         l2_policy="working set (276 MB bf16 weights + activations) far exceeds the 50 MB L2 of an H100; no explicit flush")
     if verify is not None:
         res["verify"] = verify
     del model, optimizer
@@ -592,14 +620,14 @@ def run_bert(c):
         for i in range(n):
             yield host[i % n_host]
 
-    res = measure(c, "bert", train_step, dev_batch, host_batches, None, bs, "samples/s", finish)
+    res = measure(c, "bert", train_step, dev_batch, host_batches, None, bs, "samples/s", finish, params=model.parameters)
     if args.impl != "ddp":
         res["comm_timeline"] = timeline_probe(c, model, train_step, dev_batch, finish)
     res["metric"] = f"BERT-large SQuAD-shaped fine-tuning throughput ({algo})"
     res["config"] = dict(cfg, model="bert-large (24 layers, hidden 1024, 16 heads, 335 M parameters) + QA head" if not cpu else "tiny bert (selftest)",
                          global_batch=bs * world, per_gpu_batch=bs, seq_len=seq, parallelism=f"dp{world}", algorithm=algo,
                          reference_config="examples/squad/README.md:19-28 (seq 384, bs 6/GPU, lr 3e-5)",
-                         l2_policy="670 MB of bf16 weights + 4 GB of optimizer state per step far exceed the 126 MB L2; no explicit flush")
+                         l2_policy="670 MB of bf16 weights + 4 GB of optimizer state per step far exceed the 50 MB L2 of an H100; no explicit flush")
     del model, optimizer
     return res
 
@@ -629,12 +657,15 @@ def main():
         os.environ["MASTER_ADDR"] = "127.0.0.1"
         os.environ["MASTER_PORT"] = str(find_free_network_port())
     os.environ.setdefault("LOCAL_WORLD_SIZE", str(world))
+    if args.dump_outputs:   # deterministic mode (below) needs cuBLAS's fixed workspace split, set before its first handle exists
+        os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
     # A benchmark run should fail in minutes, not hang: in-kernel cross-GPU spins and the scheduler watchdog give up earlier than the
     # training defaults (300 s); both are fatal and reported, and the line below still carries the workloads that completed.
     os.environ.setdefault("BAGUA_PEER_TIMEOUT_S", "120")
     os.environ.setdefault("BAGUA_COMM_TIMEOUT_S", "150")
 
     c = make_ctx(args)
+    c.dumps = {}
     torch = c.torch
     c.sampler = ClockSampler(c.local_rank).start() if (c.rank == 0 and not c.cpu) else None
     if args.impl == "ddp":
@@ -644,7 +675,12 @@ def main():
         import bagua_b200 as bagua
 
         bagua.init_process_group()
-    torch.backends.cudnn.benchmark = True
+    # --dump-outputs: deterministic mode, so that two runs or two builds dump the same bits. Without it the outputs drift apart far
+    # beyond rounding within the run's ~30 steps (float atomics and timing-based cuDNN algorithm choice in VGG16's backward; the
+    # attention backward, amplified by the 8-bit ByteGrad exchange and Adam, in BERT). It is slower, so such a run is not a
+    # throughput run; without the flag the benchmark measures the configuration a user runs.
+    torch.backends.cudnn.benchmark = not args.dump_outputs
+    torch.utils.deterministic.fill_uninitialized_memory = False   # deterministic mode's NaN fill of new memory: work, no reproducibility
 
     results = {}
     workloads = [w.strip() for w in args.workloads.split(",") if w.strip()]
@@ -652,6 +688,9 @@ def main():
     for wl in workloads:
         if wl not in ("vgg16", "resnet50", "bert"):
             raise SystemExit(f"unknown workload {wl}")
+        # strict for BERT (its attention backward is deterministic only then); warn-only for the CNNs, whose adaptive average pool
+        # (an identity at 224², one addend per element) has no deterministic backward and would raise
+        torch.use_deterministic_algorithms(bool(args.dump_outputs), warn_only=wl != "bert")
         try:
             results[wl] = run_bert(c) if wl == "bert" else run_cnn(c, wl)
             if not c.cpu:
@@ -666,6 +705,12 @@ def main():
             traceback.print_exc(file=sys.stderr)
             results[wl] = {"error": f"{type(e).__name__}: {e}"[:600]}
 
+    if c.rank == 0 and args.dump_outputs:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k, v in c.dumps.items():
+            np.save(os.path.join(args.dump_outputs, f"{k}.npy"), v.astype(np.float32))
     if c.rank == 0:
         first = next(iter(results))
         head = results.get("vgg16", results[first])

@@ -102,7 +102,7 @@ if rank == 0:
         os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
         with open(args.out, "w") as f:
             json.dump({"world": world, "dtype": args.dtype, "multicast": eng.has_multicast, "clocks": sampler.stop(),
-                       "roofline_note": "an all-reduce moves ~bytes in and ~bytes out of every GPU: the NVLink bound is ALGBW <= 900 GB/s nominal per direction (770 GB/s measured peer copy); busbw is reported for comparison with nccl-tests only",
+                       "roofline_note": "an all-reduce moves ~bytes in and ~bytes out of every GPU: the NVLink bound is ALGBW <= 450 GB/s nominal per direction on H100 (NVLink 4); busbw is reported for comparison with nccl-tests only",
                        "results": results}, f, indent=1)
 assert eng.comm.error_code() == 0
 dist.barrier()

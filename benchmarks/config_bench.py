@@ -3,7 +3,7 @@
   bert_bytegrad           BERT-large, SQuAD-shaped synthetic batches (seq 384), ByteGrad
   resnet50_decentralized  ResNet-50, DecentralizedAlgorithm(peer_selection_mode=all)
   resnet50_async          ResNet-50, AsyncModelAverageAlgorithm
-  gpt2_moe                GPT-2 medium MoE-8, expert all-to-all (peer dispatch/combine + tcgen05 expert GEMMs)
+  gpt2_moe                GPT-2 medium MoE-8, expert all-to-all (peer dispatch/combine + wgmma expert GEMMs)
 
 ``BAGUA_ALLREDUCE_VARIANT=nccl BAGUA_MOE_PEER=0`` runs the same schedule on NCCL/cuBLAS only (the baseline arm)."""
 import argparse

@@ -1,5 +1,4 @@
-"""tcgen05 grouped GEMM vs cuBLAS (torch.bmm) on MoE expert shapes; CUDA-event timing after warm-up, L2 flushed between calls.
-``BAGUA_GEMM_2CTA=1`` selects the cta_group::2 kernel (256x256 tiles per CTA pair) where M and N are multiples of 256."""
+"""wgmma grouped GEMM vs cuBLAS (torch.bmm) on MoE expert shapes; CUDA-event timing after warm-up, L2 flushed between calls."""
 import argparse
 import json
 import os
@@ -38,7 +37,7 @@ for (G, M, N, K) in [(1, 8192, 4096, 1024), (1, 8192, 1024, 4096), (2, 8192, 409
     flops = 2.0 * G * M * N * K
     t_ours = bench(lambda: grouped_gemm_tn(a, b, bias))
     t_cublas = bench(lambda: torch.baddbmm(bias.unsqueeze(1), a, b.transpose(1, 2)))
-    rows.append({"variant": "2cta" if os.environ.get("BAGUA_GEMM_2CTA") == "1" else "1cta", "G": G, "M": M, "N": N, "K": K, "tcgen05_ms": t_ours, "tcgen05_tflops": flops / t_ours / 1e9, "cublas_ms": t_cublas,
+    rows.append({"G": G, "M": M, "N": N, "K": K, "wgmma_ms": t_ours, "wgmma_tflops": flops / t_ours / 1e9, "cublas_ms": t_cublas,
                  "cublas_tflops": flops / t_cublas / 1e9})
     print(rows[-1])
 if args.out:

@@ -12,7 +12,7 @@ warm-up over ``--warmup-epochs`` (:562-581), top-1 / top-5 on the validation set
 the latest checkpoint, the async algorithm resumed / aborted around every epoch (:326-334), ``--prof N`` wraps iterations in
 NVTX ranges and brackets N..N+10 with cudaProfilerStart/Stop.
 
-B200-first differences: parameters and activations are bf16 channels-last by default (``--dtype fp32`` restores the reference's
+H100-first differences: parameters and activations are bf16 channels-last by default (``--dtype fp32`` restores the reference's
 precision; ``--amp`` keeps fp32 parameters and runs the forward under bf16 autocast — no loss scaling needed, bf16 has fp32's
 exponent range); batches are staged through pinned memory on a side stream (``bagua_b200.utils.data.DevicePrefetcher``) instead of
 a blocking ``.cuda()`` in the loop; ``--fused-shard`` runs SGD inside the bucket kernels (reduce-scatter → update → all-gather).

@@ -1,8 +1,6 @@
 #!/usr/bin/env bash
-# The three arms of bench.py on N GPUs of one node, one torchrun each, every command under its own timeout — how the files
-# profiles/r2/bench_n{N}_{ours,nccl_baseline,ddp}.json were produced:
-#   gpurun --gpus N --timeout 900 -- 'bash scripts/bench_arms.sh N'
-# An N-GPU call is charged N x wall time: keep multi-GPU pytest out of the same call (run `-k` subsets separately).
+# The three arms of bench.py on N GPUs of one node, one torchrun each, every command under its own timeout:
+#   bash scripts/bench_arms.sh N
 set -uo pipefail
 N=${1:-1}
 out=gpurun_out/arms_n$N

@@ -6,14 +6,15 @@
 #   bash scripts/ci/benchmark_ci.sh [NGPUS]            # GPUs of this node (default: all visible)
 #   BAGUA_CI_CPU=1 bash scripts/ci/benchmark_ci.sh 2   # plumbing run on the host (gloo, MNIST-sized model, no floors)
 #
-# Floors are per-GPU img/s for ResNet-50 bs 32 bf16 on B200 (see profiles/README.md §5 for the measured values they derive from;
-# the reference's floors — 185/180/150/115/190/165 on an unnamed 2019 GPU in fp32 — are kept below for context).
+# Floors are per-GPU img/s for ResNet-50 bs 32 bf16; they are 0 (throughput unchecked, the final loss still is) until they can be
+# derived from a measured H100 run (the reference's floors — 185/180/150/115/190/165 on an unnamed 2019 GPU in fp32 — are kept
+# below for context).
 set -uo pipefail
 cd "$(dirname "$0")/../.."
 N=${1:-$(python -c "import torch; print(max(torch.cuda.device_count(), 1))")}
 CPU=${BAGUA_CI_CPU:-0}
 algorithms=(gradient_allreduce bytegrad decentralized low_precision_decentralized async qadam)
-floors=(2300 2100 2300 1800 2300 1900)         # B200, bf16, ~0.8 x measured
+floors=(0 0 0 0 0 0)                           # not measured on H100 yet
 ref_floors=(185.0 180.0 150.0 115.0 190 165)    # reference CI (context)
 fail=()
 port=29610
@@ -32,6 +33,7 @@ for i in "${!algorithms[@]}"; do
   speed=$(grep "Img/sec per GPU" "$log" | tail -n 1 | awk '{print $4}')
   loss=$(grep "Final loss" "$log" | tail -n 1 | awk '{print $NF}')
   echo "[$a] rc=$rc img/s/GPU=${speed:-?} final_loss=${loss:-?} (floor ${floors[$i]}; reference CI floor ${ref_floors[$i]})"
+  [ "$CPU" != "1" ] && [ "${floors[$i]}" = "0" ] && echo "[$a] WARNING: no H100 throughput floor set yet: throughput is NOT checked, only the final loss"
   [ "$rc" -ne 0 ] && fail+=("$a: exit code $rc (log $log)")
   python - "$speed" "$loss" "${floors[$i]}" "$CPU" <<'PY' || fail+=("$a: throughput / loss check failed")
 import math, sys

@@ -13,7 +13,6 @@ one)
   timeout 600 python -m pytest tests -m "gpu and not multigpu" -x -q > gpurun_out/pytest_gpu_1.log 2>&1; echo "pytest1 exit=$?" | tee -a gpurun_out/plan_one.txt
   timeout 600 bash scripts/ncu_profile.sh; echo "ncu exit=$?" | tee -a gpurun_out/plan_one.txt
   BAGUA_EXPERIMENTAL=1 timeout 400 python -m pytest tests/test_zz_new_kernels_gpu.py -x -q > gpurun_out/pytest_new_kernels.log 2>&1; echo "new kernels exit=$?" | tee -a gpurun_out/plan_one.txt
-  BAGUA_GEMM_2CTA=1 timeout 200 python benchmarks/gemm_bench.py --out gpurun_out/gemm_bench_2cta.json > gpurun_out/gemm_bench_2cta.log 2>&1; echo "gemm 2cta exit=$?" | tee -a gpurun_out/plan_one.txt
   timeout 120 python benchmarks/torch_ddp_baseline.py --steps 30 --warmup 5 > gpurun_out/torch_ddp_n1.json 2> gpurun_out/torch_ddp_n1.err; echo "torch ddp baseline exit=$?" | tee -a gpurun_out/plan_one.txt
   timeout 120 python bench.py --steps 30 --warmup 5 > gpurun_out/bench1.json 2> gpurun_out/bench1.err; echo "bench exit=$?" | tee -a gpurun_out/plan_one.txt
   # A/B of the host-overhead experiment (only meaningful if the gated test above passed)

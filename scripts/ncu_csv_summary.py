@@ -32,17 +32,17 @@ def main(path):
     for k, name in COLS.items():
         c = [i for i, h in enumerate(hdr) if h == name]
         ix[k] = c[0] if c else None
-    peak = 6588.7
+    peak = 3350.0  # GB/s, H100 SXM data sheet; MEASURED_PEAKS.json overrides
     try:
         peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
     except Exception:  # noqa: BLE001
         pass
     name_i, grid_i, block_i = hdr.index("Kernel Name"), hdr.index("Grid Size"), hdr.index("Block Size")
-    print("# ncu captures of the hand-written kernels (B200, `ncu --set full --clock-control none`, one launch each, cold L2)\n")
+    print("# ncu captures of the hand-written kernels (H100, `ncu --set full --clock-control none`, one launch each, cold L2)\n")
     print(f"Source: `{os.path.relpath(path, ROOT)}` — exported on the GPU box by `scripts/ncu_zoo.sh` from one `scripts/kernel_zoo.py` run (world = 1: the peer")
     print("kernels run with this GPU as their only peer, so their loads/stores land in local HBM; ncu serialises kernels and cannot wrap a multi-rank job).")
     print(f"`HBM frac` = (DRAM bytes read + written) / duration / {peak:.1f} GB/s (measured copy peak, MEASURED_PEAKS.json). Durations under ncu are cold-cache, single")
-    print("launch; the event-timed numbers (L2 flushed, median of 5, clocks recorded) are in `profiles/r2/kernel_zoo_events_n1.jsonl`.\n")
+    print("launch; event-timed numbers (L2 flushed, median of 5, clocks recorded) come from `scripts/kernel_zoo.py`.\n")
     print("| kernel | grid x block | regs | dur µs | DRAM rd MB | DRAM wr MB | achieved GB/s | HBM frac | DRAM % | L2 % | SM % | warps active % | tensor pipe % |")
     print("|---|---|---|---|---|---|---|---|---|---|---|---|---|")
     for r in body:

@@ -11,9 +11,7 @@ NCU="ncu --set full --clock-control none --import-source on"
 # 1. fused optimizer + NHWC epilogues inside the flagship step
 $NCU -k regex:flat_sgd_kernel -s 3 -c 1 -o gpurun_out/ncu_flat_sgd python bench.py --steps 2 --warmup 3 --no-e2e > gpurun_out/ncu_flat_sgd.log 2>&1 || true
 $NCU -k regex:bias_relu_bwd_kernel -s 8 -c 1 -o gpurun_out/ncu_bias_relu_bwd python bench.py --steps 2 --warmup 3 --no-e2e > gpurun_out/ncu_bias_relu_bwd.log 2>&1 || true
-# 2. tcgen05 grouped GEMM
+# 2. wgmma grouped GEMM
 $NCU -k regex:grouped_gemm_tn_kernel -s 3 -c 1 -o gpurun_out/ncu_gemm python benchmarks/gemm_bench.py > gpurun_out/ncu_gemm.log 2>&1 || true
-# 2b. the cta_group::2 variant (only once its gated numerics test has passed)
-BAGUA_GEMM_2CTA=1 $NCU -k regex:grouped_gemm_tn_2cta_kernel -s 3 -c 1 -o gpurun_out/ncu_gemm_2cta python benchmarks/gemm_bench.py > gpurun_out/ncu_gemm_2cta.log 2>&1 || true
 # 3. every launch of one flagship step with its device time
 ncu --metrics gpu__time_duration.sum --clock-control none -s 3000 -c 400 --csv --log-file gpurun_out/launches_step.csv python bench.py --steps 2 --warmup 3 --no-e2e > gpurun_out/launches_step.log 2>&1 || true

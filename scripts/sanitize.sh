@@ -9,7 +9,7 @@ for tool in memcheck racecheck synccheck; do
   echo "$tool exit=$?" | tee -a gpurun_out/sanitizer_summary.txt
 done
 # the peer / quantised / MoE kernels among virtual ranks on this one GPU (memcheck + synccheck; racecheck only tracks shared memory and
-# does not model tcgen05 / mbarrier / cross-stream global traffic). P = 1 cases keep the run short; spinning multi-stream cases are slow under
+# does not model wgmma / mbarrier / cross-stream global traffic). P = 1 cases keep the run short; spinning multi-stream cases are slow under
 # the sanitizer, so their in-kernel time-out is raised.
 for tool in memcheck synccheck; do
   BAGUA_PEER_TIMEOUT_S=600 compute-sanitizer --tool $tool --error-exitcode 1 python -m pytest tests/test_virtual_peer_gpu.py -q -x -k "1-" \

@@ -7,5 +7,5 @@ FILTER='UTCHMMA|UTCBAR|LDTM|UTMALDG|UBLKCP|UTCATOMSWS|SYNCS|UCGABAR|LDGMC|STG\.E
 cuobjdump -sass bagua_b200/_C.so | awk -v pat="$PAT" '/Function : /{p = ($0 ~ pat)} p' > /tmp/sass_one.txt
 NAME=$(grep -m1 "Function : " /tmp/sass_one.txt | sed 's/.*Function : //')
 echo "// $NAME"
-echo "// filtered SASS (cuobjdump -sass, sm_100a): lines matching $FILTER"
+echo "// filtered SASS (cuobjdump -sass, sm_90a): lines matching $FILTER"
 grep -E "$FILTER" /tmp/sass_one.txt | sed -E 's/^\s+//' | cut -c1-150

@@ -1,6 +1,6 @@
 """Packaging for bagua_b200.
 
-The native core is built IN-TREE by ``bagua_b200/_build.py`` (nvcc -gencode arch=compute_100a,code=sm_100a; no torch
+The native core is built IN-TREE by ``bagua_b200/_build.py`` (nvcc -gencode arch=compute_90a,code=sm_90a; no torch
 headers), so ``pip install -e .`` / ``python setup.py build_ext --inplace`` only has to call it.  The reference
 packages a Rust core through setuptools_rust and downloads NCCL at install time (setup.py:60-109 of the reference);
 nothing here touches the network.
@@ -25,7 +25,7 @@ def _native_build(verbose: bool = True) -> None:
 
 
 class BuildNative(Command):
-    description = "compile bagua_b200/_C.so (and the optional NCCL net plugin) for sm_100a"
+    description = "compile bagua_b200/_C.so (and the optional NCCL net plugin) for sm_90a"
     user_options = [("inplace", "i", "kept for `build_ext --inplace` compatibility (the build is always in-tree)")]
 
     def initialize_options(self):
@@ -49,7 +49,7 @@ class BuildPyWithNative(build_py):
 setup(
     name="bagua-b200",
     version="0.1.0",
-    description="Blackwell-native distributed training engine with the capabilities of BaguaSys/bagua",
+    description="Hopper-native distributed training engine with the capabilities of BaguaSys/bagua",
     packages=find_packages(include=["bagua_b200*", "bagua", "bagua.*", "bagua_core*"]),
     package_data={"bagua_b200": ["_C.so", "_C_torch.so", "libnccl-net-bagua.so", "*.stamp", "csrc/*", "csrc/net/*", "csrc/torch_hooks/*"]},
     python_requires=">=3.10",

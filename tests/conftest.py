@@ -9,7 +9,7 @@ if REPO not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs at least one CUDA GPU (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs at least one CUDA GPU (run on the H100 box)")
     config.addinivalue_line("markers", "multigpu: test needs at least two CUDA GPUs")
     # build the native core once (incremental; a no-op when bagua_b200/_C.so is current)
     from bagua_b200 import _build

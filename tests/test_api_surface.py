@@ -1,6 +1,8 @@
 """Public API surface parity (SURVEY Appendix A): names importable through ``bagua.torch_api`` / ``bagua_core`` exactly as
 user code of the reference expects, tensor/bucket patch methods, multiple models in one process."""
 import copy
+import json
+import os
 
 import pytest
 import torch
@@ -142,39 +144,33 @@ _NOT_APPLICABLE = {
 }
 
 
-def test_every_public_name_of_the_reference_python_package_resolves():
-    """Walk the reference's python package (when it is mounted) and require each public top-level class / function to exist
-    under the same module path in the ``bagua`` alias package."""
-    import ast
-    import importlib
-    import os
+REFERENCE_API = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_api.json")
 
-    root = "/root/reference/bagua"
-    if not os.path.isdir(root):
-        pytest.skip("reference tree not mounted")
+
+def _reference_api() -> dict:
+    """Public names and parameter lists of every module of the reference's python package, stored as golden data
+    (``scripts/reference_api_golden.py`` extracts them from a checkout of the reference)."""
+    with open(REFERENCE_API) as f:
+        return json.load(f)["modules"]
+
+
+def test_every_public_name_of_the_reference_python_package_resolves():
+    """Each public top-level class / function of the reference's python package exists under the same module path in the
+    ``bagua`` alias package."""
+    import importlib
+
     missing = []
-    for d, _, files in os.walk(root):
-        for f in files:
-            if not f.endswith(".py"):
-                continue
-            path = os.path.join(d, f)
-            mod = os.path.relpath(path, "/root/reference")[:-3].replace("/", ".")
-            mod = mod[: -len(".__init__")] if mod.endswith(".__init__") else mod
-            if mod.startswith("bagua.script") or mod.startswith("bagua.distributed"):
-                continue  # CLI entry points: covered by tests/test_launchers.py
-            try:
-                tree = ast.parse(open(path).read())
-            except SyntaxError:
-                continue
-            names = [n.name for n in tree.body if isinstance(n, (ast.FunctionDef, ast.ClassDef)) and not n.name.startswith("_")]
-            try:
-                m = importlib.import_module(mod)
-            except Exception as e:  # noqa: BLE001
-                missing.append(f"{mod}: import failed: {e!r}")
-                continue
-            for n in names:
-                if not hasattr(m, n) and n not in _NOT_APPLICABLE.get(mod, ()):
-                    missing.append(f"{mod}.{n}")
+    for mod, api in sorted(_reference_api().items()):
+        if mod.startswith("bagua.script") or mod.startswith("bagua.distributed"):
+            continue  # CLI entry points: covered by tests/test_launchers.py
+        try:
+            m = importlib.import_module(mod)
+        except Exception as e:  # noqa: BLE001
+            missing.append(f"{mod}: import failed: {e!r}")
+            continue
+        for n in api["names"]:
+            if not hasattr(m, n) and n not in _NOT_APPLICABLE.get(mod, ()):
+                missing.append(f"{mod}.{n}")
     assert not missing, missing
 
 
@@ -294,10 +290,11 @@ REFERENCE_MODULES = [
 
 
 def test_every_module_path_of_the_reference_package_imports():
-    """All 49 python modules of the reference's ``bagua`` package (the list is /root/reference/bagua/**/*.py) exist under the same
+    """All 49 python modules of the reference's ``bagua`` package (the modules of tests/golden/reference_api.json) exist under the same
     dotted path in the alias package, so ``import bagua.torch_api.contrib.cache_loader`` style imports in user code keep working."""
     import importlib
 
+    assert sorted(REFERENCE_MODULES) == sorted(_reference_api())
     missing = []
     for name in REFERENCE_MODULES:
         try:
@@ -393,56 +390,37 @@ def test_sampler_and_cache_compat_methods():
 
 
 def test_public_signatures_accept_the_reference_parameter_names():
-    """Every public function / method of the reference's python package (when the tree is mounted) can be called here with the
-    reference's parameter NAMES in the reference's ORDER — keyword call sites in user code keep working."""
-    import ast
+    """Every public function / method of the reference's python package can be called here with the reference's parameter
+    NAMES in the reference's ORDER — keyword call sites in user code keep working."""
     import importlib
     import inspect
-    import os
 
-    root = "/root/reference/bagua"
-    if not os.path.isdir(root):
-        pytest.skip("reference tree not mounted")
     allowed = {("bagua.torch_api.algorithms.gradient_allreduce", "GradientAllReduceAlgorithmImpl.init_operations")}   # the reference names it "_"
     problems, checked = [], 0
-    for d, _, files in os.walk(root):
-        for f in files:
-            if not f.endswith(".py"):
+    for mod, api in sorted(_reference_api().items()):
+        try:
+            m = importlib.import_module(mod)
+        except Exception:  # noqa: BLE001 - import gaps are the business of the tests above
+            continue
+        for name, ref in api["signatures"].items():
+            obj = m
+            for part in name.split("."):
+                obj = getattr(obj, part, None)
+                if obj is None:
+                    break
+            if obj is None or (mod, name) in allowed:
                 continue
-            path = os.path.join(d, f)
-            mod = os.path.relpath(path, "/root/reference")[:-3].replace("/", ".")
-            mod = mod[: -len(".__init__")] if mod.endswith(".__init__") else mod
             try:
-                m = importlib.import_module(mod)
-                tree = ast.parse(open(path).read())
-            except Exception:  # noqa: BLE001 - import gaps are the business of the tests above
+                params = list(inspect.signature(obj).parameters.values())
+            except (TypeError, ValueError):
                 continue
-            items = []
-            for n in tree.body:
-                if isinstance(n, ast.FunctionDef) and not n.name.startswith("_"):
-                    items.append((n.name, n))
-                elif isinstance(n, ast.ClassDef) and not n.name.startswith("_"):
-                    items += [(f"{n.name}.{k.name}", k) for k in n.body if isinstance(k, ast.FunctionDef) and (k.name == "__init__" or not k.name.startswith("_"))]
-            for name, node in items:
-                obj = m
-                for part in name.split("."):
-                    obj = getattr(obj, part, None)
-                    if obj is None:
-                        break
-                if obj is None or (mod, name) in allowed:
-                    continue
-                try:
-                    params = list(inspect.signature(obj).parameters.values())
-                except (TypeError, ValueError):
-                    continue
-                ref = [a.arg for a in node.args.posonlyargs + node.args.args if a.arg not in ("self", "cls")]
-                ours = [p.name for p in params if p.name not in ("self", "cls")]
-                takes_kwargs = any(p.kind == p.VAR_KEYWORD for p in params)
-                missing = [a for a in ref if a not in ours and not takes_kwargs]
-                positional = [p.name for p in params if p.kind in (p.POSITIONAL_ONLY, p.POSITIONAL_OR_KEYWORD) and p.name not in ("self", "cls")]
-                if missing or [a for a in ref if a in positional] != [a for a in positional if a in ref]:
-                    problems.append(f"{mod}.{name}: reference {ref}, here {ours}")
-                checked += 1
+            ours = [p.name for p in params if p.name not in ("self", "cls")]
+            takes_kwargs = any(p.kind == p.VAR_KEYWORD for p in params)
+            missing = [a for a in ref if a not in ours and not takes_kwargs]
+            positional = [p.name for p in params if p.kind in (p.POSITIONAL_ONLY, p.POSITIONAL_OR_KEYWORD) and p.name not in ("self", "cls")]
+            if missing or [a for a in ref if a in positional] != [a for a in positional if a in ref]:
+                problems.append(f"{mod}.{name}: reference {ref}, here {ours}")
+            checked += 1
     assert not problems, problems
     assert checked > 150
 

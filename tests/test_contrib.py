@@ -293,7 +293,7 @@ def test_redis_store_logic_with_a_fake_redis_module(monkeypatch):
 
 
 def test_fused_op_entry_points_fall_back_on_cpu():
-    """ops.nhwc / ops.gemm front-ends on tensors the sm_100a kernels do not cover (CPU, fp32): plain torch results and gradients."""
+    """ops.nhwc / ops.gemm front-ends on tensors the sm_90a kernels do not cover (CPU, fp32): plain torch results and gradients."""
     from bagua_b200.ops.gemm import grouped_linear
     from bagua_b200.ops.nhwc import bias_relu, bias_relu_maxpool2, conv_bias_relu
 
@@ -594,7 +594,7 @@ def test_fused_linear_combine_autograd_with_a_host_double_of_the_peer_kernels():
     """``ops.moe_peer.linear_combine`` (fc2 GEMM whose epilogue does the MoE combine): its hand-written backward — scatter of
     grad·gate to the owners, dgrad / wgrad GEMMs, bias and gate-weight gradients — against plain autograd over
     ``Σ_k gate[s,k] · (x·wᵀ + b)[expert, slot]``.  The two peer kernels are replaced by single-rank torch implementations of
-    their contracts (csrc/moe_kernels.cu scatter, gemm_tcgen05.cu PEER epilogue + local-layout gather)."""
+    their contracts (csrc/moe_kernels.cu scatter, gemm_wgmma.cu PEER epilogue + local-layout gather)."""
     from bagua_b200.ops import moe_peer
 
     class HostContext(moe_peer.MoEPeerContext):

@@ -1,4 +1,4 @@
-"""Single-GPU numerics of the sm_100a kernels against plain PyTorch fp32 references."""
+"""Single-GPU numerics of the sm_90a kernels against plain PyTorch fp32 references."""
 import pytest
 import torch
 
@@ -165,7 +165,7 @@ def test_flagship_smoke(dev):
     ge.smoke()
 
 
-@pytest.mark.parametrize("G,M,N,K", [(1, 128, 128, 64), (2, 256, 384, 192), (4, 1024, 512, 1024)])
+@pytest.mark.parametrize("G,M,N,K", [(1, 128, 128, 64), (2, 256, 384, 192), (4, 1024, 512, 1024), (4, 2048, 1024, 256)])  # last: 256 tiles > 132 SMs
 def test_tcgen05_grouped_gemm_matches_fp32_reference(dev, G, M, N, K):
     from bagua_b200.ops.gemm import grouped_gemm_tn, grouped_linear
 
@@ -235,3 +235,30 @@ def test_vgg16_fused_path_matches_module_path(dev):
         res.append((out.detach().float(), m.features[0].bias.grad.float().clone(), m.features[28].weight.grad.float().clone()))
     for a, b in zip(*res):
         torch.testing.assert_close(a, b, rtol=5e-2, atol=5e-2 * max(1.0, b.abs().max().item()))
+
+
+@pytest.mark.parametrize("pool", [False, True])
+def test_nhwc_bias_grad_is_reproducible_in_deterministic_mode(dev, pool):
+    """Under torch.use_deterministic_algorithms the bias gradient is the same bits on every call and agrees with the kernel's own
+    (atomic, order-varying) reduction of the default mode."""
+    from bagua_b200.ops.nhwc import bias_relu, bias_relu_maxpool2
+
+    torch.manual_seed(8)
+    C, H = 128, 32
+    x = torch.randn(8, C, H, H, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    g = torch.randn(8, C, H // 2 if pool else H, H // 2 if pool else H, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    fn = bias_relu_maxpool2 if pool else bias_relu
+
+    def bias_grad():
+        b = torch.randn(C, device=dev, generator=torch.Generator(device=dev).manual_seed(3)).to(torch.bfloat16).requires_grad_(True)
+        fn(x.clone(), b).backward(g)
+        return b.grad.float()
+
+    default = bias_grad()
+    torch.use_deterministic_algorithms(True, warn_only=True)
+    try:
+        runs = [bias_grad() for _ in range(3)]
+    finally:
+        torch.use_deterministic_algorithms(False)
+    assert all(torch.equal(runs[0], r) for r in runs[1:])
+    torch.testing.assert_close(runs[0], default, rtol=2e-2, atol=2e-2 * default.abs().max().item())

@@ -181,7 +181,7 @@ def test_bagua_doctor_reports_and_self_tests():
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
     rep = json.loads(r.stdout[r.stdout.index("{"):])
     assert rep["ok"] and all(t["ok"] for t in rep["self_test"]) and len(rep["self_test"]) >= 2
-    assert rep["libraries"]["_C.so (native core, sm_100a kernels)"]["current_with_sources"] is True
+    assert rep["libraries"]["_C.so (native core, sm_90a kernels)"]["current_with_sources"] is True
     assert rep["environment"]["BAGUA_DEFAULT_BUCKET_SIZE"] == "1048576" and rep["gpus"]["count"] == 0
 
 

@@ -1,10 +1,14 @@
-"""Executable model of the mbarrier protocol of the tcgen05 GEMM kernels (csrc/gemm_tcgen05.cu): the warp roles are coroutines,
-the barriers follow the PTX semantics (arrival count, expect_tx / complete_tx byte credit, phase parity), asynchronous agents
-(TMA, the tensor core's in-order completion queue) act after random delays, and a random scheduler interleaves everything.
-Checked over many schedules and shapes: no deadlock, a waiter is never lapped by its barrier (parity ambiguity), no shared
-memory stage is overwritten before the MMAs that read it have completed, no accumulator is overwritten before all epilogue
-warps have drained it, every tile is produced exactly once.  The 2-CTA variant (cta_group::2: leader-owned ``full`` and
-``acc_empty`` barriers, multicast commits) is the one that has not run on hardware yet; the 1-CTA model is the control."""
+"""Executable models of warp-specialised GEMM mbarrier protocols: the warp roles are coroutines, the barriers follow the PTX
+semantics (arrival count, expect_tx / complete_tx byte credit, phase parity), asynchronous agents (TMA, the tensor core's in-order
+completion queues) act after random delays, and a random scheduler interleaves everything.  Checked over many schedules and
+shapes: no deadlock, a waiter is never lapped by its barrier (parity ambiguity), no shared-memory stage is overwritten before the
+MMAs that read it have completed, every tile is produced exactly once.
+
+``WgmmaModel`` is the protocol of csrc/gemm_wgmma.cu: one TMA producer, two consumer warpgroups that each issue a wgmma group per
+stage, keep one group in flight (``wgmma.wait_group 1``) and only then release the PREVIOUS stage, ``empty`` armed with one
+arrival per consumer warpgroup.  ``Model`` is a design this code base no longer ships (a dedicated MMA issuer whose commits
+release stages, double-buffered tensor-memory accumulators, 1-CTA and 2-CTA forms); it is kept as a check of the barrier
+arithmetic shared by both."""
 import random
 
 import pytest
@@ -205,6 +209,122 @@ def test_model_detects_a_wrong_arrival_count():
         m.acc_empty = [Barrier(4) for _ in range(2)]
         try:
             m.run()
+        except AssertionError:
+            failures += 1
+    assert failures > 0
+
+
+class Until:
+    def __init__(self, cond):
+        self.cond = cond
+
+    def ready(self):
+        return self.cond()
+
+
+class WgmmaModel:
+    """csrc/gemm_wgmma.cu: full[s] (1 arrival + expect_tx), empty[s] (``empty_count`` arrivals, 2 in the kernel)."""
+
+    def __init__(self, stages, tiles, num_kb, seed, empty_count=2):
+        self.rng = random.Random(seed)
+        self.S, self.tiles, self.num_kb = stages, tiles, num_kb
+        self.full = [Barrier(1) for _ in range(stages)]
+        self.empty = [Barrier(empty_count) for _ in range(stages)]
+        self.smem = [None] * stages          # (tile, kb) resident in stage s
+        self.reads = [0] * stages            # wgmma groups still reading stage s
+        self.groups = [[], []]               # per consumer warpgroup: stages of its outstanding groups, completed in order
+        self.async_q = []
+        self.done = [[], []]
+
+    def step_agents(self):
+        progressed = False
+        for item in list(self.async_q):
+            progressed = True
+            if item[0] <= 0:
+                self.async_q.remove(item)
+                item[1]()
+            else:
+                item[0] -= 1
+        for q in self.groups:
+            if q and self.rng.random() < 0.5:
+                self.reads[q.pop(0)] -= 1
+                progressed = True
+        return progressed
+
+    def producer(self):
+        it = 0
+        for tile in range(self.tiles):
+            for kb in range(self.num_kb):
+                s, k = it % self.S, it // self.S
+                yield wait_parity(self.empty[s], (k & 1) ^ 1, k - 1)
+                self.full[s].expect_tx(A_BYTES + B_BYTES)
+
+                def land(s=s, tile=tile, kb=kb):
+                    assert self.reads[s] == 0, "TMA overwrote a stage that a wgmma group still reads"
+                    self.smem[s] = (tile, kb)
+                    self.full[s].complete_tx(A_BYTES + B_BYTES)
+
+                self.async_q.append([self.rng.randint(0, 6), land])
+                it += 1
+                yield None
+
+    def consumer(self, cw):
+        it = 0
+        for tile in range(self.tiles):
+            prev = None
+            for kb in range(self.num_kb):
+                s = it % self.S
+                yield wait_parity(self.full[s], (it // self.S) & 1, it // self.S)
+                assert self.smem[s] == (tile, kb), f"consumer {cw} expects {(tile, kb)} in stage {s}, finds {self.smem[s]}"
+                self.reads[s] += 1
+                self.groups[cw].append(s)                                   # wgmma x4 + commit_group
+                yield Until(lambda cw=cw: len(self.groups[cw]) <= 1)        # wait_group 1: the previous group is done
+                if prev is not None:
+                    self.empty[prev].arrive()
+                prev = s
+                it += 1
+            yield Until(lambda cw=cw: not self.groups[cw])                 # wait_group 0
+            self.empty[prev].arrive()
+            for _ in range(self.rng.randint(0, 3)):
+                yield None                                                  # epilogue from registers
+            self.done[cw].append(tile)
+
+    def run(self):
+        actors = [self.producer(), self.consumer(0), self.consumer(1)]
+        blocked = {id(a): None for a in actors}
+        live, idle_rounds = list(actors), 0
+        while live:
+            progressed = self.step_agents()
+            self.rng.shuffle(live)
+            for a in list(live):
+                w = blocked[id(a)]
+                if w is not None and not w.ready():
+                    continue
+                try:
+                    blocked[id(a)] = next(a)
+                except StopIteration:
+                    live.remove(a)
+                progressed = True
+            idle_rounds = 0 if (progressed or self.async_q or any(self.groups)) else idle_rounds + 1
+            assert idle_rounds < 3, "deadlock: every warp role is blocked and no asynchronous work is pending"
+        assert self.done == [list(range(self.tiles))] * 2
+
+
+@pytest.mark.parametrize("stages", [4, 6])
+def test_wgmma_stage_ring_has_no_deadlock_or_hazard(stages):
+    rng = random.Random(stages)
+    for seed in range(200):
+        tiles, num_kb = rng.randint(1, 7), rng.choice([1, 2, 3, stages - 1, stages, stages + 1, 16])
+        WgmmaModel(stages, tiles, num_kb, seed).run()
+
+
+def test_wgmma_model_detects_a_single_arrival_empty_barrier():
+    """With ``empty`` armed for one arrival the first consumer to release a stage would let TMA overwrite it while the other
+    consumer's wgmma group still reads it."""
+    failures = 0
+    for seed in range(60):
+        try:
+            WgmmaModel(4, 4, 6, seed, empty_count=1).run()
         except AssertionError:
             failures += 1
     assert failures > 0

@@ -521,3 +521,31 @@ def test_a_lonely_collective_times_out_and_poisons_the_communicator(C):
     w2.comms[0].abort()
     torch.cuda.synchronize()
     assert w2.comms[0].error_code() == 2
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# grouped GEMM whose epilogue is the MoE combine: every 128-row tile lands in the buffer of the rank that sent those rows
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("P", [1, 2, 4])
+def test_grouped_gemm_push_stores_each_source_tile_on_its_owner(C, P):
+    w = _world(P)
+    G, cap, K = 2, 256, 128
+    gen = torch.Generator(device="cpu").manual_seed(60 + P)
+    for N, act in ((256, 0), (384, 1)):                      # BN = 256 and BN = 128 instantiations, plain and GELU epilogue
+        out_bytes = P * G * cap * N * 2
+        buf = w.alloc(out_bytes)
+        A = [(torch.randn(G, P * cap, K, generator=gen) * 0.5).to(torch.bfloat16).cuda() for _ in range(P)]   # rows [source rank][slot]
+        B = [(torch.randn(G, N, K, generator=gen) * 0.5).to(torch.bfloat16).cuda() for _ in range(P)]
+        bias = [torch.randn(G, N, generator=gen).cuda() for _ in range(P)]
+        w.launch_all(lambda r, st: C.grouped_gemm_tn_push(A[r].data_ptr(), B[r].data_ptr(), bias[r].data_ptr(), G, N, K, act, w.comms[r], buf.buf, 0,
+                                                          cap, st))
+        torch.cuda.synchronize()
+        for r in range(P):
+            ref = torch.bmm(A[r].float(), B[r].float().transpose(1, 2)) + bias[r].unsqueeze(1)
+            if act == 1:
+                ref = torch.nn.functional.gelu(ref, approximate="tanh")
+            for s in range(P):                                # owner s holds, at [r][g][slot], what expert g of rank r made of s's rows
+                got = buf.view(s, torch.bfloat16, P * G * cap * N).view(P, G, cap, N)[r].float()
+                want = ref[:, s * cap:(s + 1) * cap]
+                torch.testing.assert_close(got, want, rtol=2e-2, atol=2e-2 * want.abs().max().item())
+    w.check()
