@@ -13,6 +13,7 @@
 #include <string>
 
 #include "bulk_pipe.cuh"
+#include "dispatch.h"
 #include "kernels.h"
 #include "peer.cuh"
 #include "quant.cuh"
@@ -436,36 +437,6 @@ __global__ void __launch_bounds__(512) lpdec_ring_kernel(PeerCtx ctx, T* x, T* w
 }
 
 // ---------------------------------------------------------------------------------------------------------
-namespace {
-template <typename F>
-void dispatch_world(int world, F&& f) {
-    switch (world) {
-        case 1: f(std::integral_constant<int, 1>{}); break;
-        case 2: f(std::integral_constant<int, 2>{}); break;
-        case 4: f(std::integral_constant<int, 4>{}); break;
-        case 8: f(std::integral_constant<int, 8>{}); break;
-        case 3: f(std::integral_constant<int, 3>{}); break;
-        case 5: f(std::integral_constant<int, 5>{}); break;
-        case 6: f(std::integral_constant<int, 6>{}); break;
-        case 7: f(std::integral_constant<int, 7>{}); break;
-        default: throw std::runtime_error("bagua: peer kernels support 1..8 ranks, got " + std::to_string(world));
-    }
-}
-template <typename F>
-void dispatch_float(int dtype, F&& f) {
-    switch (dtype) {
-        case F32: f(float{}); break;
-        case F16: f(__half{}); break;
-        case BF16: f(__nv_bfloat16{}); break;
-        default: throw std::runtime_error("bagua: quantised collectives need f32/f16/bf16, got dtype code " + std::to_string(dtype));
-    }
-}
-void check(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) throw std::runtime_error(std::string("bagua: launch of ") + what + " failed: " + cudaGetErrorString(e));
-    count_launch();
-}
-}  // namespace
 
 // Host-side bookkeeping of a scratch instance: returns {sequence number, arrival base} for this launch and
 // advances both (n_barriers grid barriers of nblocks arrivals each).
@@ -513,7 +484,7 @@ void launch_bytegrad(const PeerCtx& ctx, void* data, size_t numel, int dtype, co
     if (numel % (static_cast<size_t>(P) * 32)) throw std::runtime_error("bagua: bytegrad bucket must be a multiple of 32*nranks elements");
     if (nblocks % P || nblocks < P || nblocks > kMaxCommBlocks) throw std::runtime_error("bagua: bytegrad grid must be a multiple of nranks (≤ 256)");
     size_t chunk = numel / P;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "quantised collectives", [&](auto tag) {
         using T = decltype(tag);
         dispatch_world(P, [&](auto pw) {
             constexpr int PP = decltype(pw)::value;
@@ -538,7 +509,7 @@ void launch_bytegrad(const PeerCtx& ctx, void* data, size_t numel, int dtype, co
             launch_grid_synced(kernel, nb, nthreads, stream, args, smem);
         });
     });
-    check("bytegrad");
+    check_launch("bytegrad");
 }
 
 void launch_lpdec_ring(const PeerCtx& ctx, void* x, void* w, void* l, void* r, size_t numel, int dtype, const PeerBuf& box,
@@ -546,7 +517,7 @@ void launch_lpdec_ring(const PeerCtx& ctx, void* x, void* w, void* l, void* r, s
                        cudaStream_t stream) {
     if (numel % 32) throw std::runtime_error("bagua: low-precision ring bucket must be a multiple of 32 elements");
     if (nblocks < 1 || nblocks > kMaxCommBlocks) throw std::runtime_error("bagua: bad grid for lpdec ring");
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "quantised collectives", [&](auto tag) {
         using T = decltype(tag);
         auto kernel = lpdec_ring_kernel<T>;
         const int nb = clamp_grid_to_residency(kernel, nblocks, nthreads, 1);
@@ -559,7 +530,7 @@ void launch_lpdec_ring(const PeerCtx& ctx, void* x, void* w, void* l, void* r, s
         void* args[] = {&c, &xx, &ww, &ll, &rr, &numel, &bx, &box_off, &sc, &seq, &base, &left, &right};
         launch_grid_synced(kernel, nb, nthreads, stream, args);
     });
-    check("lpdec_ring");
+    check_launch("lpdec_ring");
 }
 
 }  // namespace bagua

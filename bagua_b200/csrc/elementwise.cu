@@ -5,6 +5,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "dispatch.h"
 #include "kernels.h"
 #include "quant.cuh"
 
@@ -18,20 +19,6 @@ inline int grid_for(size_t work_items, int per_thread = 4, int max_blocks = 132 
     if (b < 1) b = 1;
     if (b > static_cast<size_t>(max_blocks)) b = max_blocks;
     return static_cast<int>(b);
-}
-void check(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) throw std::runtime_error(std::string("bagua: launch of ") + what + " failed: " + cudaGetErrorString(e));
-    count_launch();
-}
-template <typename F>
-void dispatch_float(int dtype, F&& f) {
-    switch (dtype) {
-        case F32: f(float{}); break;
-        case F16: f(__half{}); break;
-        case BF16: f(__nv_bfloat16{}); break;
-        default: throw std::runtime_error("bagua: kernel needs f32/f16/bf16, got dtype code " + std::to_string(dtype));
-    }
 }
 }  // namespace
 
@@ -104,12 +91,12 @@ void launch_minmax_uint8_compress(const void* in, size_t numel, int dtype, int n
     auto* mm = reinterpret_cast<uint32_t*>(minmax_scratch);
     minmax_init_kernel<<<(2 * n_chunks + 255) / 256, 256, 0, stream>>>(mm, 2 * n_chunks);
     dim3 grid(grid_for(chunk, 8, 132 * 4 / (count > 4 ? 4 : 1)), count);
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "elementwise kernels", [&](auto tag) {
         using T = decltype(tag);
         chunk_minmax_kernel<T><<<grid, kThreads, 0, stream>>>(static_cast<const T*>(in), chunk, first, mm);
         chunk_quantize_kernel<T><<<grid, kThreads, 0, stream>>>(static_cast<const T*>(in), chunk, chunk_bytes, first, mm, out);
     });
-    check("minmax_uint8_compress");
+    check_launch("minmax_uint8_compress");
     count_launch(2);  // init + min/max + quantise = 3 launches
 }
 
@@ -118,11 +105,11 @@ void launch_minmax_uint8_decompress(const uint8_t* in, size_t numel, int dtype, 
     const size_t chunk = numel / n_chunks;
     if (chunk == 0) return;
     dim3 grid(grid_for(chunk, 8, 132 * 4 / (n_chunks > 4 ? 4 : 1)), n_chunks);
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "elementwise kernels", [&](auto tag) {
         using T = decltype(tag);
         chunk_dequantize_kernel<T><<<grid, kThreads, 0, stream>>>(in, chunk, minmax_uint8_chunk_bytes(chunk), static_cast<T*>(out));
     });
-    check("minmax_uint8_decompress");
+    check_launch("minmax_uint8_decompress");
 }
 
 // ---- element-wise family ---------------------------------------------------------------------------------
@@ -136,12 +123,12 @@ __global__ void __launch_bounds__(kThreads) async_apply_kernel(T* __restrict__ w
 
 void launch_async_apply(void* w, const void* red, const void* snap, size_t numel, int dtype, float inv_p, cudaStream_t stream) {
     if (!numel) return;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "elementwise kernels", [&](auto tag) {
         using T = decltype(tag);
         async_apply_kernel<T><<<grid_for(numel), kThreads, 0, stream>>>(static_cast<T*>(w), static_cast<const T*>(red),
                                                                        static_cast<const T*>(snap), numel, inv_p);
     });
-    check("async_apply");
+    check_launch("async_apply");
 }
 
 template <typename T>
@@ -158,12 +145,12 @@ __global__ void __launch_bounds__(kThreads) reduce_chunks_kernel(T* __restrict__
 void launch_reduce_chunks(void* data, size_t chunk_elems, int n_chunks, int target_chunk, int dtype, bool average,
                           cudaStream_t stream) {
     if (!chunk_elems) return;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "elementwise kernels", [&](auto tag) {
         using T = decltype(tag);
         reduce_chunks_kernel<T><<<grid_for(chunk_elems), kThreads, 0, stream>>>(static_cast<T*>(data), chunk_elems, n_chunks,
                                                                                 target_chunk, average ? 1.0f / n_chunks : 1.0f);
     });
-    check("reduce_chunks");
+    check_launch("reduce_chunks");
 }
 
 template <typename T>
@@ -175,11 +162,11 @@ __global__ void __launch_bounds__(kThreads) axpby_kernel(T* __restrict__ x, cons
 
 void launch_axpby(void* x, const void* y, size_t numel, int dtype, float a, float b, cudaStream_t stream) {
     if (!numel) return;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "elementwise kernels", [&](auto tag) {
         using T = decltype(tag);
         axpby_kernel<T><<<grid_for(numel), kThreads, 0, stream>>>(static_cast<T*>(x), static_cast<const T*>(y), numel, a, b);
     });
-    check("axpby");
+    check_launch("axpby");
 }
 
 template <typename T>
@@ -191,11 +178,11 @@ __global__ void __launch_bounds__(kThreads) scale_kernel(T* __restrict__ x, size
 
 void launch_scale(void* x, size_t numel, int dtype, float a, cudaStream_t stream) {
     if (!numel) return;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "elementwise kernels", [&](auto tag) {
         using T = decltype(tag);
         scale_kernel<T><<<grid_for(numel), kThreads, 0, stream>>>(static_cast<T*>(x), numel, a);
     });
-    check("scale");
+    check_launch("scale");
 }
 
 template <typename TI, typename TO>
@@ -207,14 +194,14 @@ __global__ void __launch_bounds__(kThreads) cast_kernel(const TI* __restrict__ i
 
 void launch_cast(const void* in, int in_dtype, void* out, int out_dtype, size_t numel, cudaStream_t stream) {
     if (!numel) return;
-    dispatch_float(in_dtype, [&](auto ti) {
+    dispatch_float(in_dtype, "elementwise kernels", [&](auto ti) {
         using TI = decltype(ti);
-        dispatch_float(out_dtype, [&](auto to) {
+        dispatch_float(out_dtype, "elementwise kernels", [&](auto to) {
             using TO = decltype(to);
             cast_kernel<TI, TO><<<grid_for(numel), kThreads, 0, stream>>>(static_cast<const TI*>(in), static_cast<TO*>(out), numel);
         });
     });
-    check("cast");
+    check_launch("cast");
 }
 
 }  // namespace bagua

@@ -8,6 +8,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "dispatch.h"
 #include "kernels.h"
 #include "peer.cuh"
 
@@ -148,20 +149,6 @@ __global__ void __launch_bounds__(kMoeThreads)
 }
 
 namespace {
-template <typename F>
-void dispatch_float(int dtype, F&& f) {
-    switch (dtype) {
-        case F32: f(float{}); break;
-        case F16: f(__half{}); break;
-        case BF16: f(__nv_bfloat16{}); break;
-        default: throw std::runtime_error("bagua: MoE kernels need f32/f16/bf16, got dtype code " + std::to_string(dtype));
-    }
-}
-void check(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) throw std::runtime_error(std::string("bagua: launch of ") + what + " failed: " + cudaGetErrorString(e));
-    count_launch();
-}
 void check_shape(int M, int dtype, int nblocks) {
     if ((static_cast<size_t>(M) * dtype_size(dtype)) % 16) throw std::runtime_error("bagua: MoE rows must be a multiple of 16 bytes");
     if (nblocks < 1 || nblocks > kMaxCommBlocks) throw std::runtime_error("bagua: bad grid for MoE kernel");
@@ -175,24 +162,24 @@ void launch_moe_scatter(const PeerCtx& ctx, const PeerBuf& dst, size_t dst_off, 
     const size_t bytes = static_cast<size_t>(ctx.world) * E_local * C * M * dtype_size(dtype);
     cudaError_t me = cudaMemsetAsync(dst.ptr[ctx.rank] + dst_off, 0, bytes, stream);
     if (me != cudaSuccess) throw std::runtime_error(std::string("bagua: moe_scatter memset failed: ") + cudaGetErrorString(me));
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "MoE kernels", [&](auto tag) {
         using T = decltype(tag);
         moe_scatter_kernel<T><<<nblocks, kMoeThreads, 0, stream>>>(ctx, dst, dst_off, static_cast<const T*>(rows_in), expert_idx, slot_idx, scale, S, K,
                                                                   M, E_local, C);
     });
-    check("moe_scatter");
+    check_launch("moe_scatter");
 }
 
 void launch_moe_gather(const PeerCtx& ctx, const PeerBuf& src, size_t src_off, void* out, const int64_t* expert_idx, const int64_t* slot_idx,
                        const float* weights, void* picked, int S, int K, int M, int E_local, int C, int dtype, int nblocks,
                        cudaStream_t stream, bool local_layout) {
     check_shape(M, dtype, nblocks);
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "MoE kernels", [&](auto tag) {
         using T = decltype(tag);
         moe_gather_kernel<T><<<nblocks, kMoeThreads, 0, stream>>>(ctx, src, src_off, static_cast<T*>(out), expert_idx, slot_idx, weights,
                                                                  static_cast<T*>(picked), S, K, M, E_local, C, local_layout ? 1 : 0);
     });
-    check("moe_gather");
+    check_launch("moe_gather");
 }
 
 }  // namespace bagua

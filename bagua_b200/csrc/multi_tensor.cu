@@ -9,6 +9,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "dispatch.h"
 #include "kernels.h"
 #include "quant.cuh"
 
@@ -18,12 +19,6 @@ using namespace dev;
 namespace {
 constexpr int kThreads = 512;
 constexpr int kVec = 8;  // elements per thread per iteration
-
-void check(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) throw std::runtime_error(std::string("bagua: launch of ") + what + " failed: " + cudaGetErrorString(e));
-    count_launch();
-}
 
 template <typename T>
 struct alignas(sizeof(T) * kVec) Pack {
@@ -73,15 +68,6 @@ inline int flat_grid(size_t numel) {
     return static_cast<int>(b);
 }
 
-template <typename F>
-void dispatch_float(int dtype, F&& f) {
-    switch (dtype) {
-        case F32: f(float{}); break;
-        case F16: f(__half{}); break;
-        case BF16: f(__nv_bfloat16{}); break;
-        default: throw std::runtime_error("bagua: optimizer kernels need f32/f16/bf16, got dtype code " + std::to_string(dtype));
-    }
-}
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 31u) == 0; }  // packs of 8 fp32 = 32 B
 }  // namespace
 
@@ -129,9 +115,9 @@ void launch_flat_sgd(void* param, int param_dtype, const void* grad, int grad_dt
     if (hp.momentum != 0.f && !momentum_buf) throw std::runtime_error("bagua: flat_sgd with momentum needs a momentum buffer");
     const bool vec = aligned16(param) && aligned16(grad) && (!momentum_buf || aligned16(momentum_buf)) && (!model || aligned16(model));
     const int grid = flat_grid(numel);
-    dispatch_float(param_dtype, [&](auto pt) {
+    dispatch_float(param_dtype, "optimizer kernels", [&](auto pt) {
         using PT = decltype(pt);
-        dispatch_float(grad_dtype, [&](auto gt) {
+        dispatch_float(grad_dtype, "optimizer kernels", [&](auto gt) {
             using GT = decltype(gt);
             auto* g = const_cast<GT*>(static_cast<const GT*>(grad));
             auto launch = [&](auto mt, auto has_model) {
@@ -155,7 +141,7 @@ void launch_flat_sgd(void* param, int param_dtype, const void* grad, int grad_dt
             }
         });
     });
-    check("flat_sgd");
+    check_launch("flat_sgd");
 }
 
 // ---- flat Adam / AdamW ----------------------------------------------------------------------------------------
@@ -205,9 +191,9 @@ void launch_flat_adam(void* param, int param_dtype, const void* grad, int grad_d
     if (hp.amsgrad) throw std::runtime_error("bagua: flat_adam does not implement amsgrad");
     const bool vec = aligned16(param) && aligned16(grad) && aligned16(exp_avg) && aligned16(exp_avg_sq) && (!model || aligned16(model));
     const int grid = flat_grid(numel);
-    dispatch_float(param_dtype, [&](auto pt) {
+    dispatch_float(param_dtype, "optimizer kernels", [&](auto pt) {
         using PT = decltype(pt);
-        dispatch_float(grad_dtype, [&](auto gt) {
+        dispatch_float(grad_dtype, "optimizer kernels", [&](auto gt) {
             using GT = decltype(gt);
             auto* g = const_cast<GT*>(static_cast<const GT*>(grad));
             auto launch = [&](auto mt, auto has_model) {
@@ -231,7 +217,7 @@ void launch_flat_adam(void* param, int param_dtype, const void* grad, int grad_d
             }
         });
     });
-    check("flat_adam");
+    check_launch("flat_adam");
 }
 
 // ---- multi-tensor (non-contiguous) variants -------------------------------------------------------------------
@@ -298,33 +284,33 @@ __global__ void __launch_bounds__(kThreads) multi_tensor_adam_mp_kernel(TensorLi
 
 void launch_multi_tensor_adam_mp(const TensorListDesc& d, int dtype, const AdamParams& hp, float grad_scale, cudaStream_t stream) {
     if (d.n_blocks <= 0) return;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
         using T = decltype(tag);
         multi_tensor_adam_mp_kernel<T><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, grad_scale);
     });
-    check("multi_tensor_adam_mp");
+    check_launch("multi_tensor_adam_mp");
 }
 
 void launch_multi_tensor_sgd(const TensorListDesc& d, int dtype, bool has_momentum, const SgdParams& hp, float grad_scale,
                              cudaStream_t stream) {
     if (d.n_blocks <= 0) return;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
         using T = decltype(tag);
         if (has_momentum)
             multi_tensor_sgd_kernel<T, true><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, grad_scale);
         else
             multi_tensor_sgd_kernel<T, false><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, grad_scale);
     });
-    check("multi_tensor_sgd");
+    check_launch("multi_tensor_sgd");
 }
 
 void launch_multi_tensor_adam(const TensorListDesc& d, int dtype, const AdamParams& hp, float grad_scale, cudaStream_t stream) {
     if (d.n_blocks <= 0) return;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
         using T = decltype(tag);
         multi_tensor_adam_kernel<T><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, grad_scale);
     });
-    check("multi_tensor_adam");
+    check_launch("multi_tensor_adam");
 }
 
 // ---- QAdam momentum pre-step -------------------------------------------------------------------------------------
@@ -337,11 +323,11 @@ __global__ void __launch_bounds__(kThreads) qadam_momentum_kernel(float* __restr
 
 void launch_qadam_momentum(float* exp_avg, const void* grad, int grad_dtype, size_t numel, float beta1, cudaStream_t stream) {
     if (!numel) return;
-    dispatch_float(grad_dtype, [&](auto tag) {
+    dispatch_float(grad_dtype, "optimizer kernels", [&](auto tag) {
         using GT = decltype(tag);
         qadam_momentum_kernel<GT><<<flat_grid(numel), kThreads, 0, stream>>>(exp_avg, static_cast<const GT*>(grad), numel, beta1);
     });
-    check("qadam_momentum");
+    check_launch("qadam_momentum");
 }
 
 }  // namespace bagua

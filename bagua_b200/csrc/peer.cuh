@@ -164,10 +164,27 @@ __device__ __forceinline__ void raise_error(const PeerCtx& ctx, int code) {
 }
 
 // ---- cross-GPU barrier ----------------------------------------------------------------------------------
+// Spins with acquire loads until the flag reaches `epoch` (epochs only grow, so no reset pass and no ABA). The spin is
+// bounded: every 1024 spins it checks the host-mapped abort flag (PeerComm.abort()) and the timeout; on either it raises
+// ctx.error and returns false.
+__device__ __forceinline__ bool spin_until_epoch(const PeerCtx& ctx, const uint32_t* flag, uint32_t epoch) {
+    unsigned long long t0 = 0;
+    uint32_t spins = 0;
+    while (static_cast<int32_t>(ld_acquire_sys(flag) - epoch) < 0) {
+        if ((++spins & 0x3ff) == 0) {
+            unsigned long long now = globaltimer_ns();
+            if (t0 == 0) t0 = now;
+            if (*ctx.abort != 0 || now - t0 > ctx.timeout_ns) {
+                raise_error(ctx, *ctx.abort != 0 ? 2 : 1);
+                return false;
+            }
+        }
+    }
+    return true;
+}
+
 // Every CTA b of every rank owns flag row b. Thread p (< world) publishes `epoch` into rank p's slot
-// [b][my_rank] with a system-scope release and spins with acquire loads on its own slot [b][p].
-// Epochs only grow, so no reset pass and no ABA. The spin is bounded: a host-mapped abort flag
-// (PeerComm.abort()) or a timeout makes the kernel give up, raise ctx.error and return false.
+// [b][my_rank] with a system-scope release and spins on its own slot [b][p]. Returns false if the spin gave up.
 __device__ __forceinline__ bool peer_barrier(const PeerCtx& ctx, uint32_t epoch) {
     __shared__ int s_ok;
     if (threadIdx.x == 0) s_ok = 1;
@@ -176,20 +193,7 @@ __device__ __forceinline__ bool peer_barrier(const PeerCtx& ctx, uint32_t epoch)
         const int p = threadIdx.x;
         uint32_t* remote = ctx.flags[p] + blockIdx.x * kFlagStride + ctx.rank;
         st_release_sys(remote, epoch);
-        const uint32_t* mine = ctx.flags[ctx.rank] + blockIdx.x * kFlagStride + p;
-        unsigned long long t0 = 0;
-        uint32_t spins = 0;
-        while (static_cast<int32_t>(ld_acquire_sys(mine) - epoch) < 0) {
-            if ((++spins & 0x3ff) == 0) {
-                unsigned long long now = globaltimer_ns();
-                if (t0 == 0) t0 = now;
-                if (*ctx.abort != 0 || now - t0 > ctx.timeout_ns) {
-                    raise_error(ctx, *ctx.abort != 0 ? 2 : 1);
-                    s_ok = 0;
-                    break;
-                }
-            }
-        }
+        if (!spin_until_epoch(ctx, ctx.flags[ctx.rank] + blockIdx.x * kFlagStride + p, epoch)) s_ok = 0;
     }
     __syncthreads();
     return s_ok != 0;
@@ -208,23 +212,10 @@ __device__ __forceinline__ bool peer_barrier_vote(const PeerCtx& ctx, uint32_t e
         const int p = threadIdx.x;
         asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(ctx.flags[p] + kVoteWordOffset + ctx.rank), "r"(my_word) : "memory");
         st_release_sys(ctx.flags[p] + blockIdx.x * kFlagStride + ctx.rank, epoch);
-        const uint32_t* mine = ctx.flags[ctx.rank] + blockIdx.x * kFlagStride + p;
-        unsigned long long t0 = 0;
-        uint32_t spins = 0;
-        bool ok = true;
-        while (static_cast<int32_t>(ld_acquire_sys(mine) - epoch) < 0) {
-            if ((++spins & 0x3ff) == 0) {
-                unsigned long long now = globaltimer_ns();
-                if (t0 == 0) t0 = now;
-                if (*ctx.abort != 0 || now - t0 > ctx.timeout_ns) {
-                    raise_error(ctx, *ctx.abort != 0 ? 2 : 1);
-                    s_ok_v = 0;
-                    ok = false;
-                    break;
-                }
-            }
-        }
-        if (ok) s_votes[p] = ld_relaxed_sys(ctx.flags[ctx.rank] + kVoteWordOffset + p);
+        if (spin_until_epoch(ctx, ctx.flags[ctx.rank] + blockIdx.x * kFlagStride + p, epoch))
+            s_votes[p] = ld_relaxed_sys(ctx.flags[ctx.rank] + kVoteWordOffset + p);
+        else
+            s_ok_v = 0;
     }
     __syncthreads();
     return s_ok_v != 0;

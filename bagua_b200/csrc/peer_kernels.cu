@@ -4,11 +4,111 @@
 // (rust/bagua-core/bagua-core-internal/src/comm_ops/*.rs, communicators/mod.rs:1121-1153): the reduction,
 // the averaging scale, the dtype handling, the optimizer update and the data movement to/from the peers
 // happen in ONE kernel that issues peer (P2P) or NVLS multicast loads/stores itself.
+#include "dispatch.h"
 #include "kernels.h"
 #include "peer.cuh"
 
 namespace bagua {
 using namespace dev;
+
+// ---------------------------------------------------------------------------------------------------------
+// How a buffer of `total` 16-byte vectors is cut into `world` slices — rank r owns vectors [r·vpr, min((r+1)·vpr, total)) — and
+// this thread's place in the grid-stride loops over them. A kernel builds it once, where it first needs it, and every phase reuses it.
+struct Slicing {
+    size_t total, vpr, tid, stride;
+    __device__ __forceinline__ Slicing(size_t total_vecs, int world)
+        : total(total_vecs),
+          vpr((total_vecs + world - 1) / world),
+          tid(static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x),
+          stride(static_cast<size_t>(gridDim.x) * blockDim.x) {}
+};
+
+// The owned-slice schedule every reduction kernel runs. Each thread walks its share of slice `rank` grid-stride, U vectors per
+// iteration, and issues every load of an iteration before it consumes any: U·P independent 16-byte peer loads in flight per thread
+// is what keeps NVLink busy (NVLink latency is ~2 us: bandwidth = bytes in flight / latency, measured 7.5 GB/s per CTA without
+// unrolling). load(raw, v) fills one Raw for vector v; consume(raw, v, j) gets it back with j = v − base, the index in the shard.
+// ---------------------------------------------------------------------------------------------------------
+template <int U, typename Raw, typename Load, typename Consume>
+__device__ __forceinline__ void walk_owned_slice(const Slicing& sl, int rank, Load&& load, Consume&& consume) {
+    const size_t base = static_cast<size_t>(rank) * sl.vpr;
+    const size_t limit = (base + sl.vpr < sl.total ? base + sl.vpr : sl.total);  // exclusive end of my slice
+    for (size_t j0 = base + sl.tid; j0 < limit; j0 += sl.stride * U) {
+        Raw raw[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const size_t v = j0 + u * sl.stride;
+            if (v < limit) load(raw[u], v);
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const size_t v = j0 + u * sl.stride;
+            if (v < limit) consume(raw[u], v, v - base);
+        }
+    }
+}
+
+// The owned-slice reduction: for every vector v of my slice, epi(v, j, acc) receives the fp32 sum over the P ranks' copies of
+// src. The sum starts from my own copy and adds ranks rank+1, rank+2, … (mod P) in that order — the rotation also spreads the
+// loads evenly over the links — or, with USE_MC, is one multimem.ld_reduce inside the switch.
+template <typename T, int P, bool USE_MC, int U, typename Epi>
+__device__ __forceinline__ void reduce_owned_slice(const PeerCtx& ctx, const PeerBuf& src, size_t off, const Slicing& sl, Epi&& epi) {
+    using Raw = uint4[USE_MC ? 1 : P];
+    walk_owned_slice<U, Raw>(
+        sl, ctx.rank,
+        [&](Raw& raw, size_t v) {
+            if constexpr (USE_MC) {
+                raw[0] = multimem_ld_reduce_add<T>(src.mc + off + v * 16);
+            } else {
+#pragma unroll
+                for (int i = 0; i < P; ++i) raw[i] = ld_peer16(src.ptr[(ctx.rank + i) % P] + off + v * 16);
+            }
+        },
+        [&](Raw& raw, size_t v, size_t j) {
+            float acc[Vec16<T>::N];
+            Vec16<T>::unpack(raw[0], acc);
+#pragma unroll
+            for (int i = 1; i < (USE_MC ? 1 : P); ++i) {
+                float f[Vec16<T>::N];
+                Vec16<T>::unpack(raw[i], f);
+#pragma unroll
+                for (int k = 0; k < Vec16<T>::N; ++k) acc[k] += f[k];
+            }
+            epi(v, j, acc);
+        });
+}
+
+// Stores one 16-byte vector at index v of every rank's copy of dst: one multimem.st, or peer stores in the same rotated order as the
+// loads. skip_self leaves my own copy alone.
+template <int P, bool USE_MC>
+__device__ __forceinline__ void publish16(const PeerCtx& ctx, const PeerBuf& dst, size_t off, size_t v, const uint4& val, bool skip_self = false) {
+    if constexpr (USE_MC) {
+        multimem_st16(dst.mc + off + v * 16, val);
+    } else {
+#pragma unroll
+        for (int i = skip_self ? 1 : 0; i < P; ++i) st_peer16(dst.ptr[(ctx.rank + i) % P] + off + v * 16, val);
+    }
+}
+
+// Column striping: f(v) for v = s·vpr + j of every slice s, with this thread's columns j ≡ (block, thread) mod grid — the columns
+// walk_owned_slice gives it in slice s = rank. So CTA b touches the same column range of every slice in every phase, and the per-CTA
+// barriers (CTA b of every rank) are all the synchronisation the kernels need; there is no grid-wide barrier.
+template <int P, typename F>
+__device__ __forceinline__ void for_each_striped(const Slicing& sl, F&& f) {
+    for (size_t j = sl.tid; j < sl.vpr; j += sl.stride) {
+#pragma unroll
+        for (int s = 0; s < P; ++s) {
+            const size_t v = static_cast<size_t>(s) * sl.vpr + j;
+            if (v < sl.total) f(v);
+        }
+    }
+}
+
+// Vectors per thread per iteration of the pure reductions, and of the optimizer kernels, whose register budget is U·P·4 on top of
+// the optimizer state.
+template <int P, bool USE_MC>
+constexpr int kReduceUnroll = USE_MC ? 8 : (P <= 2 ? 8 : (P <= 4 ? 4 : 2));
+template <int P, bool USE_MC>
+constexpr int kOptimizerUnroll = USE_MC ? 4 : (P <= 2 ? 4 : (P <= 4 ? 2 : 1));
 
 // ---------------------------------------------------------------------------------------------------------
 // allreduce, two-shot over peer pointers: rank r reduces slice r (reading it from every peer) and writes the
@@ -18,88 +118,39 @@ using namespace dev;
 template <typename T, int P>
 __global__ void __launch_bounds__(512) allreduce_twoshot_kernel(PeerCtx ctx, PeerBuf src, PeerBuf dst, size_t src_off,
                                                                 size_t dst_off, size_t total_vecs, float scale) {
-    // U vectors per thread per iteration keep U*P independent 16-byte peer loads in flight (NVLink latency is ~2 us:
-    // bandwidth = bytes in flight / latency, measured 7.5 GB/s per CTA without unrolling)
-    constexpr int U = P <= 2 ? 8 : (P <= 4 ? 4 : 2);
     const uint32_t e0 = load_epoch(ctx);
     bool ok = peer_barrier(ctx, e0 + 1);
     if (ok) {
-        const size_t vpr = (total_vecs + P - 1) / P;
-        const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-        const size_t base = static_cast<size_t>(ctx.rank) * vpr;
-        const size_t limit = (base + vpr < total_vecs ? base + vpr : total_vecs);  // exclusive end of my slice
-        for (size_t j0 = base + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; j0 < limit; j0 += stride * U) {
-            uint4 raw[U][P];
+        reduce_owned_slice<T, P, false, kReduceUnroll<P, false>>(ctx, src, src_off, Slicing(total_vecs, P), [&](size_t v, size_t, float* acc) {
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) {
-#pragma unroll
-                    for (int i = 0; i < P; ++i) raw[u][i] = ld_peer16(src.ptr[(ctx.rank + i) % P] + src_off + v * 16);  // rotate: links hit evenly
-                }
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) {
-                    float acc[Vec16<T>::N];
-                    Vec16<T>::unpack(raw[u][0], acc);
-#pragma unroll
-                    for (int i = 1; i < P; ++i) {
-                        float f[Vec16<T>::N];
-                        Vec16<T>::unpack(raw[u][i], f);
-#pragma unroll
-                        for (int k = 0; k < Vec16<T>::N; ++k) acc[k] += f[k];
-                    }
-#pragma unroll
-                    for (int k = 0; k < Vec16<T>::N; ++k) acc[k] *= scale;
-                    const uint4 out = Vec16<T>::pack(acc);
-#pragma unroll
-                    for (int i = 0; i < P; ++i) st_peer16(dst.ptr[(ctx.rank + i) % P] + dst_off + v * 16, out);
-                }
-            }
-        }
+            for (int k = 0; k < Vec16<T>::N; ++k) acc[k] *= scale;
+            publish16<P, false>(ctx, dst, dst_off, v, Vec16<T>::pack(acc));
+        });
         peer_barrier(ctx, e0 + 2);
     }
     store_epoch(ctx, e0 + 2);
 }
 
 // Same schedule through the switch: one multimem.ld_reduce returns the sum over all GPUs (reduced inside
-// NVSwitch), one multimem.st lands the result on all GPUs.
+// NVSwitch), one multimem.st lands the result on all GPUs. The world size is a runtime value here.
 template <typename T>
 __global__ void __launch_bounds__(512) allreduce_multimem_kernel(PeerCtx ctx, PeerBuf src, PeerBuf dst, size_t src_off,
                                                                  size_t dst_off, size_t total_vecs, float scale) {
-    constexpr int U = 8;  // independent in-switch reductions in flight per thread
     const uint32_t e0 = load_epoch(ctx);
     bool ok = peer_barrier(ctx, e0 + 1);
     if (ok) {
-        const int P = ctx.world;
-        const size_t vpr = (total_vecs + P - 1) / P;
-        const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-        const size_t base = static_cast<size_t>(ctx.rank) * vpr;
-        const size_t limit = (base + vpr < total_vecs ? base + vpr : total_vecs);
-        for (size_t j0 = base + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; j0 < limit; j0 += stride * U) {
-            uint4 red[U];
+        walk_owned_slice<8, uint4>(
+            Slicing(total_vecs, ctx.world), ctx.rank, [&](uint4& red, size_t v) { red = multimem_ld_reduce_add<T>(src.mc + src_off + v * 16); },
+            [&](uint4& red, size_t v, size_t) {
+                if (scale != 1.0f) {  // only then: unpacking and repacking may change NaN payloads
+                    float f[Vec16<T>::N];
+                    Vec16<T>::unpack(red, f);
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) red[u] = multimem_ld_reduce_add<T>(src.mc + src_off + v * 16);
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) {
-                    if (scale != 1.0f) {
-                        float f[Vec16<T>::N];
-                        Vec16<T>::unpack(red[u], f);
-#pragma unroll
-                        for (int k = 0; k < Vec16<T>::N; ++k) f[k] *= scale;
-                        red[u] = Vec16<T>::pack(f);
-                    }
-                    multimem_st16(dst.mc + dst_off + v * 16, red[u]);
+                    for (int k = 0; k < Vec16<T>::N; ++k) f[k] *= scale;
+                    red = Vec16<T>::pack(f);
                 }
-            }
-        }
+                multimem_st16(dst.mc + dst_off + v * 16, red);
+            });
         peer_barrier(ctx, e0 + 2);
     }
     store_epoch(ctx, e0 + 2);
@@ -115,49 +166,15 @@ __global__ void __launch_bounds__(512) allreduce_multimem_kernel(PeerCtx ctx, Pe
 // ---------------------------------------------------------------------------------------------------------
 template <typename T, int P, bool USE_MC>
 __global__ void __launch_bounds__(512) reduce_scatter_kernel(PeerCtx ctx, PeerBuf buf, size_t off, size_t total_vecs, float scale) {
-    constexpr int U = USE_MC ? 8 : (P <= 2 ? 8 : (P <= 4 ? 4 : 2));
     const uint32_t e0 = load_epoch(ctx);
     bool ok = peer_barrier(ctx, e0 + 1);
     if (ok) {
-        const size_t vpr = (total_vecs + P - 1) / P;
-        const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-        const size_t base = static_cast<size_t>(ctx.rank) * vpr;
-        const size_t limit = (base + vpr < total_vecs ? base + vpr : total_vecs);
         char* mine = buf.ptr[ctx.rank] + off;
-        for (size_t j0 = base + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; j0 < limit; j0 += stride * U) {
-            uint4 raw[U][USE_MC ? 1 : P];
+        reduce_owned_slice<T, P, USE_MC, kReduceUnroll<P, USE_MC>>(ctx, buf, off, Slicing(total_vecs, P), [&](size_t v, size_t, float* acc) {
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) {
-                    if (USE_MC) {
-                        raw[u][0] = multimem_ld_reduce_add<T>(buf.mc + off + v * 16);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < (USE_MC ? 1 : P); ++i) raw[u][i] = ld_peer16(buf.ptr[(ctx.rank + i) % P] + off + v * 16);
-                    }
-                }
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v >= limit) continue;
-                float acc[Vec16<T>::N];
-                Vec16<T>::unpack(raw[u][0], acc);
-                if (!USE_MC) {
-#pragma unroll
-                    for (int i = 1; i < (USE_MC ? 1 : P); ++i) {
-                        float f[Vec16<T>::N];
-                        Vec16<T>::unpack(raw[u][i], f);
-#pragma unroll
-                        for (int k = 0; k < Vec16<T>::N; ++k) acc[k] += f[k];
-                    }
-                }
-#pragma unroll
-                for (int k = 0; k < Vec16<T>::N; ++k) acc[k] *= scale;
-                st_stream16(mine + v * 16, Vec16<T>::pack(acc));
-            }
-        }
+            for (int k = 0; k < Vec16<T>::N; ++k) acc[k] *= scale;
+            st_stream16(mine + v * 16, Vec16<T>::pack(acc));
+        });
         peer_barrier(ctx, e0 + 2);
     }
     store_epoch(ctx, e0 + 2);
@@ -165,34 +182,13 @@ __global__ void __launch_bounds__(512) reduce_scatter_kernel(PeerCtx ctx, PeerBu
 
 template <typename T, int P, bool USE_MC>
 __global__ void __launch_bounds__(512) all_gather_kernel(PeerCtx ctx, PeerBuf buf, size_t off, size_t total_vecs) {
-    constexpr int U = 4;
     const uint32_t e0 = load_epoch(ctx);
     bool ok = peer_barrier(ctx, e0 + 1);  // nobody is still reading the slices that are about to be overwritten
     if (ok) {
-        const size_t vpr = (total_vecs + P - 1) / P;
-        const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-        const size_t base = static_cast<size_t>(ctx.rank) * vpr;
-        const size_t limit = (base + vpr < total_vecs ? base + vpr : total_vecs);
         const char* mine = buf.ptr[ctx.rank] + off;
-        for (size_t j0 = base + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; j0 < limit; j0 += stride * U) {
-            uint4 raw[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) raw[u] = ld_stream16(mine + v * 16);
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v >= limit) continue;
-                if (USE_MC) {
-                    multimem_st16(buf.mc + off + v * 16, raw[u]);
-                } else {
-#pragma unroll
-                    for (int i = 1; i < P; ++i) st_peer16(buf.ptr[(ctx.rank + i) % P] + off + v * 16, raw[u]);  // my own copy is already in place
-                }
-            }
-        }
+        walk_owned_slice<4, uint4>(
+            Slicing(total_vecs, P), ctx.rank, [&](uint4& raw, size_t v) { raw = ld_stream16(mine + v * 16); },
+            [&](uint4& raw, size_t v, size_t) { publish16<P, USE_MC>(ctx, buf, off, v, raw, /*skip_self=*/true); });  // mine is in place
         peer_barrier(ctx, e0 + 2);  // every slice has landed everywhere
     }
     store_epoch(ctx, e0 + 2);
@@ -213,14 +209,8 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_kernel(PeerCtx ctx, Pee
     const size_t parity = (call_parity & 1u);
     const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
     const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    for (size_t v = tid; v < total_vecs; v += stride) {
-        const uint4 mine = ld_stream16(in + v * 16);
-#pragma unroll
-        for (int i = 0; i < P; ++i) {
-            const int p = (ctx.rank + i) % P;
-            st_peer16(staging.ptr[p] + staging_off + (parity * P + ctx.rank) * slot_bytes + v * 16, mine);
-        }
-    }
+    for (size_t v = tid; v < total_vecs; v += stride)
+        publish16<P, false>(ctx, staging, staging_off + (parity * P + ctx.rank) * slot_bytes, v, ld_stream16(in + v * 16));
     bool ok = peer_barrier(ctx, e0 + 1);
     if (ok) {
         const char* mystage = staging.ptr[ctx.rank] + staging_off + parity * P * slot_bytes;
@@ -255,92 +245,44 @@ __global__ void __launch_bounds__(512)
     const uint32_t e0 = load_epoch(ctx);
     bool ok = peer_barrier(ctx, e0 + 1);
     constexpr int N = Vec16<T>::N;
-    const size_t vpr = (total_vecs + P - 1) / P;
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const Slicing sl(total_vecs, P);
     if (ok) {
-        constexpr int U = USE_MC ? 4 : (P <= 2 ? 4 : (P <= 4 ? 2 : 1));  // vectors in flight per thread (register budget: U*P*4)
-        const size_t base = static_cast<size_t>(ctx.rank) * vpr;
-        const size_t limit = (base + vpr < total_vecs ? base + vpr : total_vecs);
-        for (size_t j0 = base + tid; j0 < limit; j0 += stride * U) {
-            uint4 raw[U][USE_MC ? 1 : P];
+        reduce_owned_slice<T, P, USE_MC, kOptimizerUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t v, size_t j, float* g) {
+            // optimizer state of the owned slice: index j*N within the shard
+            float w[N], m[N];
+            float4* mp = reinterpret_cast<float4*>(master + j * N);
+            float4* mo = reinterpret_cast<float4*>(momentum_buf + j * N);
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) {
-                    if (USE_MC) {
-                        raw[u][0] = multimem_ld_reduce_add<T>(grads.mc + g_off + v * 16);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < (USE_MC ? 1 : P); ++i) raw[u][i] = ld_peer16(grads.ptr[(ctx.rank + i) % P] + g_off + v * 16);
-                    }
+            for (int q = 0; q < N / 4; ++q) {
+                float4 a = mp[q];
+                w[4 * q] = a.x, w[4 * q + 1] = a.y, w[4 * q + 2] = a.z, w[4 * q + 3] = a.w;
+                if (hp.momentum != 0.f) {
+                    float4 bb = mo[q];
+                    m[4 * q] = bb.x, m[4 * q + 1] = bb.y, m[4 * q + 2] = bb.z, m[4 * q + 3] = bb.w;
                 }
             }
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v >= limit) continue;
-                const size_t j = v - base;
-                float g[N];
-                Vec16<T>::unpack(raw[u][0], g);
-                if (!USE_MC) {
-#pragma unroll
-                    for (int i = 1; i < (USE_MC ? 1 : P); ++i) {
-                        float f[N];
-                        Vec16<T>::unpack(raw[u][i], f);
-#pragma unroll
-                        for (int k = 0; k < N; ++k) g[k] += f[k];
-                    }
+            for (int k = 0; k < N; ++k) {
+                float d = g[k] * scale + hp.weight_decay * w[k];
+                if (hp.momentum != 0.f) {
+                    m[k] = hp.first_step ? d : hp.momentum * m[k] + (1.f - hp.dampening) * d;
+                    d = hp.nesterov ? d + hp.momentum * m[k] : m[k];
                 }
-                // optimizer state of the owned slice: index j*N within the shard
-                float w[N], m[N];
-                float4* mp = reinterpret_cast<float4*>(master + j * N);
-                float4* mo = reinterpret_cast<float4*>(momentum_buf + j * N);
-#pragma unroll
-                for (int q = 0; q < N / 4; ++q) {
-                    float4 a = mp[q];
-                    w[4 * q] = a.x, w[4 * q + 1] = a.y, w[4 * q + 2] = a.z, w[4 * q + 3] = a.w;
-                    if (hp.momentum != 0.f) {
-                        float4 bb = mo[q];
-                        m[4 * q] = bb.x, m[4 * q + 1] = bb.y, m[4 * q + 2] = bb.z, m[4 * q + 3] = bb.w;
-                    }
-                }
-#pragma unroll
-                for (int k = 0; k < N; ++k) {
-                    float d = g[k] * scale + hp.weight_decay * w[k];
-                    if (hp.momentum != 0.f) {
-                        m[k] = hp.first_step ? d : hp.momentum * m[k] + (1.f - hp.dampening) * d;
-                        d = hp.nesterov ? d + hp.momentum * m[k] : m[k];
-                    }
-                    w[k] -= hp.lr * d;
-                }
-#pragma unroll
-                for (int q = 0; q < N / 4; ++q) {
-                    mp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-                    if (hp.momentum != 0.f) mo[q] = make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]);
-                }
-                const uint4 out = Vec16<T>::pack(w);
-                if (USE_MC) {
-                    multimem_st16(weights.mc + w_off + v * 16, out);
-                } else {
-#pragma unroll
-                    for (int i = 0; i < P; ++i) st_peer16(weights.ptr[(ctx.rank + i) % P] + w_off + v * 16, out);
-                }
+                w[k] -= hp.lr * d;
             }
-        }
+#pragma unroll
+            for (int q = 0; q < N / 4; ++q) {
+                mp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+                if (hp.momentum != 0.f) mo[q] = make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]);
+            }
+            publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
+        });
         ok = peer_barrier(ctx, e0 + 2);
     }
     if (ok && zero_grads) {
         // Block b of every peer has finished reading column-range b of all my slices: safe to clear them.
         char* mine = grads.ptr[ctx.rank] + g_off;
-        const uint4 z = make_uint4(0, 0, 0, 0);
-        for (size_t j = tid; j < vpr; j += stride) {
-#pragma unroll
-            for (int s = 0; s < P; ++s) {
-                const size_t v = static_cast<size_t>(s) * vpr + j;
-                if (v < total_vecs) st_stream16(mine + v * 16, z);
-            }
-        }
+        for_each_striped<P>(sl, [&](size_t v) { st_stream16(mine + v * 16, make_uint4(0, 0, 0, 0)); });
     }
     store_epoch(ctx, e0 + 2);
 }
@@ -356,90 +298,42 @@ __global__ void __launch_bounds__(512)
     const uint32_t e0 = load_epoch(ctx);
     bool ok = peer_barrier(ctx, e0 + 1);
     constexpr int N = Vec16<T>::N;
-    const size_t vpr = (total_vecs + P - 1) / P;
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const Slicing sl(total_vecs, P);
     if (ok) {
-        constexpr int U = USE_MC ? 4 : (P <= 2 ? 4 : (P <= 4 ? 2 : 1));
-        const size_t base = static_cast<size_t>(ctx.rank) * vpr;
-        const size_t limit = (base + vpr < total_vecs ? base + vpr : total_vecs);
         const float inv_bc1 = 1.f / hp.bias_correction1, inv_sqrt_bc2 = rsqrtf(hp.bias_correction2);
-        for (size_t j0 = base + tid; j0 < limit; j0 += stride * U) {
-            uint4 raw[U][USE_MC ? 1 : P];
+        reduce_owned_slice<T, P, USE_MC, kOptimizerUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t v, size_t j, float* g) {
+            float4* wp = reinterpret_cast<float4*>(master + j * N);
+            float4* ap = reinterpret_cast<float4*>(exp_avg + j * N);
+            float4* bp = reinterpret_cast<float4*>(exp_avg_sq + j * N);
+            float w[N];
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) {
-                    if (USE_MC) {
-                        raw[u][0] = multimem_ld_reduce_add<T>(grads.mc + g_off + v * 16);
-                    } else {
+            for (int q = 0; q < N / 4; ++q) {
+                float4 ww = wp[q], aa = ap[q], bb = bp[q];
+                float wv[4] = {ww.x, ww.y, ww.z, ww.w}, av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
 #pragma unroll
-                        for (int i = 0; i < (USE_MC ? 1 : P); ++i) raw[u][i] = ld_peer16(grads.ptr[(ctx.rank + i) % P] + g_off + v * 16);
-                    }
+                for (int k = 0; k < 4; ++k) {
+                    float gg = g[4 * q + k] * scale;
+                    if (hp.adamw)
+                        wv[k] *= (1.f - hp.lr * hp.weight_decay);
+                    else
+                        gg += hp.weight_decay * wv[k];
+                    av[k] = hp.beta1 * av[k] + (1.f - hp.beta1) * gg;
+                    bv[k] = hp.beta2 * bv[k] + (1.f - hp.beta2) * gg * gg;
+                    const float denom = sqrtf(bv[k]) * inv_sqrt_bc2 + hp.eps;
+                    wv[k] -= (hp.lr * inv_bc1) * (av[k] / denom);
+                    w[4 * q + k] = wv[k];
                 }
+                wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
+                ap[q] = make_float4(av[0], av[1], av[2], av[3]);
+                bp[q] = make_float4(bv[0], bv[1], bv[2], bv[3]);
             }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v >= limit) continue;
-                const size_t j = v - base;
-                float g[N];
-                Vec16<T>::unpack(raw[u][0], g);
-                if (!USE_MC) {
-#pragma unroll
-                    for (int i = 1; i < (USE_MC ? 1 : P); ++i) {
-                        float f[N];
-                        Vec16<T>::unpack(raw[u][i], f);
-#pragma unroll
-                        for (int k = 0; k < N; ++k) g[k] += f[k];
-                    }
-                }
-                float4* wp = reinterpret_cast<float4*>(master + j * N);
-                float4* ap = reinterpret_cast<float4*>(exp_avg + j * N);
-                float4* bp = reinterpret_cast<float4*>(exp_avg_sq + j * N);
-                float w[N];
-#pragma unroll
-                for (int q = 0; q < N / 4; ++q) {
-                    float4 ww = wp[q], aa = ap[q], bb = bp[q];
-                    float wv[4] = {ww.x, ww.y, ww.z, ww.w}, av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        float gg = g[4 * q + k] * scale;
-                        if (hp.adamw)
-                            wv[k] *= (1.f - hp.lr * hp.weight_decay);
-                        else
-                            gg += hp.weight_decay * wv[k];
-                        av[k] = hp.beta1 * av[k] + (1.f - hp.beta1) * gg;
-                        bv[k] = hp.beta2 * bv[k] + (1.f - hp.beta2) * gg * gg;
-                        const float denom = sqrtf(bv[k]) * inv_sqrt_bc2 + hp.eps;
-                        wv[k] -= (hp.lr * inv_bc1) * (av[k] / denom);
-                        w[4 * q + k] = wv[k];
-                    }
-                    wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
-                    ap[q] = make_float4(av[0], av[1], av[2], av[3]);
-                    bp[q] = make_float4(bv[0], bv[1], bv[2], bv[3]);
-                }
-                const uint4 out = Vec16<T>::pack(w);
-                if (USE_MC) {
-                    multimem_st16(weights.mc + w_off + v * 16, out);
-                } else {
-#pragma unroll
-                    for (int i = 0; i < P; ++i) st_peer16(weights.ptr[(ctx.rank + i) % P] + w_off + v * 16, out);
-                }
-            }
-        }
+            publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
+        });
         ok = peer_barrier(ctx, e0 + 2);
     }
     if (ok && zero_grads) {
         char* mine = grads.ptr[ctx.rank] + g_off;
-        const uint4 z = make_uint4(0, 0, 0, 0);
-        for (size_t j = tid; j < vpr; j += stride) {
-#pragma unroll
-            for (int s = 0; s < P; ++s) {
-                const size_t v = static_cast<size_t>(s) * vpr + j;
-                if (v < total_vecs) st_stream16(mine + v * 16, z);
-            }
-        }
+        for_each_striped<P>(sl, [&](size_t v) { st_stream16(mine + v * 16, make_uint4(0, 0, 0, 0)); });
     }
     store_epoch(ctx, e0 + 2);
 }
@@ -490,8 +384,8 @@ __global__ void __launch_bounds__(512)
 //                        reference does not guarantee) — without any host synchronisation, and a straggling peer only
 //                        delays this background kernel, never the trainer.
 //
-// Column striping: CTA b touches vectors {s·vpr + j : j ≡ (b, thread) mod grid} of every slice s in all three phases, so the
-// per-CTA barriers (CTA b of every rank) are all the synchronisation needed; there is no grid-wide barrier.
+// All three phases are column-striped (for_each_striped, and the owned-slice walk for phase 2), so the per-CTA barriers are all
+// the synchronisation needed; there is no grid-wide barrier.
 // gate words: [0] state (0 free, 1 trainer, 2 averaging), [1] "averaging is waiting" (fairness), [2] CTAs finished,
 // [3] CTAs past the last cross-rank barrier, [4] decision of the acquiring CTA (1 apply, 2 skip).
 // ---------------------------------------------------------------------------------------------------------
@@ -509,19 +403,11 @@ __global__ void __launch_bounds__(512)
     __shared__ int s_gate;
     constexpr int N = Vec16<T>::N;
     const uint32_t e0 = load_epoch(ctx);
-    const size_t vpr = (total_vecs + P - 1) / P;
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    const size_t tid = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const Slicing sl(total_vecs, P);
     char* my_snap = snap.ptr[ctx.rank] + snap_off;
     // 1: snapshot (weights may be mid-update by the optimizer on another stream: every 16-byte vector is still a value the
     //    weight had at some instant, which is all the element-wise averaging algebra needs)
-    for (size_t j = tid; j < vpr; j += stride) {
-#pragma unroll
-        for (int s = 0; s < P; ++s) {
-            const size_t v = static_cast<size_t>(s) * vpr + j;
-            if (v < total_vecs) st_stream16(my_snap + v * 16, ld_peer16(w + v * 16));
-        }
-    }
+    for_each_striped<P>(sl, [&](size_t v) { st_stream16(my_snap + v * 16, ld_peer16(w + v * 16)); });
     bool ok = peer_barrier_vote(ctx, e0 + 1, (seq << 1) | (go ? 1u : 0u), s_votes);
     bool all_go = true;
     if (ok) {
@@ -534,50 +420,12 @@ __global__ void __launch_bounds__(512)
     }
     if (ok && all_go) {
         // 2: mean of my slice → everybody's avg buffer
-        constexpr int U = USE_MC ? 8 : (P <= 2 ? 8 : (P <= 4 ? 4 : 2));
-        const size_t base = static_cast<size_t>(ctx.rank) * vpr;
-        const size_t limit = (base + vpr < total_vecs ? base + vpr : total_vecs);
         const float inv = 1.0f / P;
-        for (size_t j0 = base + tid; j0 < limit; j0 += stride * U) {
-            uint4 raw[U][USE_MC ? 1 : P];
+        reduce_owned_slice<T, P, USE_MC, kReduceUnroll<P, USE_MC>>(ctx, snap, snap_off, sl, [&](size_t v, size_t, float* acc) {
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v < limit) {
-                    if (USE_MC) {
-                        raw[u][0] = multimem_ld_reduce_add<T>(snap.mc + snap_off + v * 16);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < (USE_MC ? 1 : P); ++i) raw[u][i] = ld_peer16(snap.ptr[(ctx.rank + i) % P] + snap_off + v * 16);
-                    }
-                }
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const size_t v = j0 + u * stride;
-                if (v >= limit) continue;
-                float acc[N];
-                Vec16<T>::unpack(raw[u][0], acc);
-                if (!USE_MC) {
-#pragma unroll
-                    for (int i = 1; i < (USE_MC ? 1 : P); ++i) {
-                        float f[N];
-                        Vec16<T>::unpack(raw[u][i], f);
-#pragma unroll
-                        for (int k = 0; k < N; ++k) acc[k] += f[k];
-                    }
-                }
-#pragma unroll
-                for (int k = 0; k < N; ++k) acc[k] *= inv;
-                const uint4 out = Vec16<T>::pack(acc);
-                if (USE_MC) {
-                    multimem_st16(avg.mc + avg_off + v * 16, out);
-                } else {
-#pragma unroll
-                    for (int i = 0; i < P; ++i) st_peer16(avg.ptr[(ctx.rank + i) % P] + avg_off + v * 16, out);
-                }
-            }
-        }
+            for (int k = 0; k < N; ++k) acc[k] *= inv;
+            publish16<P, USE_MC>(ctx, avg, avg_off, v, Vec16<T>::pack(acc));
+        });
         ok = peer_barrier(ctx, e0 + 2);
         if (ok) {
             // 3: take the weight gate — by the LAST CTA to get here, i.e. once everything that is left is local work, so the
@@ -615,20 +463,15 @@ __global__ void __launch_bounds__(512)
             __syncthreads();
             if (s_gate) {
                 const char* my_avg = avg.ptr[ctx.rank] + avg_off;
-                for (size_t j = tid; j < vpr; j += stride) {
+                for_each_striped<P>(sl, [&](size_t v) {
+                    float a[N], sn[N], cur[N];
+                    Vec16<T>::unpack(ld_peer16(my_avg + v * 16), a);       // written by the slice owner during this kernel
+                    Vec16<T>::unpack(ld_stream16(my_snap + v * 16), sn);  // written by this very thread in phase 1
+                    Vec16<T>::unpack(ld_peer16(w + v * 16), cur);         // the weights as they are NOW
 #pragma unroll
-                    for (int s = 0; s < P; ++s) {
-                        const size_t v = static_cast<size_t>(s) * vpr + j;
-                        if (v >= total_vecs) continue;
-                        float a[N], sn[N], cur[N];
-                        Vec16<T>::unpack(ld_peer16(my_avg + v * 16), a);       // written by rank s during this kernel
-                        Vec16<T>::unpack(ld_stream16(my_snap + v * 16), sn);  // written by this very thread in phase 1
-                        Vec16<T>::unpack(ld_peer16(w + v * 16), cur);         // the weights as they are NOW
-#pragma unroll
-                        for (int k = 0; k < N; ++k) cur[k] += a[k] - sn[k];
-                        st_stream16(w + v * 16, Vec16<T>::pack(cur));
-                    }
-                }
+                    for (int k = 0; k < N; ++k) cur[k] += a[k] - sn[k];
+                    st_stream16(w + v * 16, Vec16<T>::pack(cur));
+                });
             }
             if (gate != nullptr) {
                 __syncthreads();
@@ -689,54 +532,28 @@ __global__ void peer_barrier_kernel(PeerCtx ctx) {
 // host launchers
 // ---------------------------------------------------------------------------------------------------------
 namespace {
-template <typename F>
-void dispatch_world(int world, F&& f) {
-    switch (world) {
-        case 1: f(std::integral_constant<int, 1>{}); break;
-        case 2: f(std::integral_constant<int, 2>{}); break;
-        case 3: f(std::integral_constant<int, 3>{}); break;
-        case 4: f(std::integral_constant<int, 4>{}); break;
-        case 5: f(std::integral_constant<int, 5>{}); break;
-        case 6: f(std::integral_constant<int, 6>{}); break;
-        case 7: f(std::integral_constant<int, 7>{}); break;
-        case 8: f(std::integral_constant<int, 8>{}); break;
-        default: throw std::runtime_error("bagua: peer kernels support 1..8 ranks, got " + std::to_string(world));
-    }
-}
-template <typename F>
-void dispatch_float(int dtype, F&& f) {
-    switch (dtype) {
-        case F32: f(float{}); break;
-        case F16: f(__half{}); break;
-        case BF16: f(__nv_bfloat16{}); break;
-        default: throw std::runtime_error("bagua: peer reduction kernels need f32/f16/bf16, got dtype code " + std::to_string(dtype));
-    }
-}
-void check_launch(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) throw std::runtime_error(std::string("bagua: launch of ") + what + " failed: " + cudaGetErrorString(e));
-    count_launch();
-}
-void check_blocks(int nblocks) {
+constexpr const char* kFamily = "peer reduction kernels";
+
+// The checks every peer launcher makes; returns the number of 16-byte vectors to process.
+size_t peer_vecs(const char* what, size_t bytes, size_t off_a, size_t off_b, int nblocks) {
+    if ((bytes | off_a | off_b) % 16) throw std::runtime_error(std::string("bagua: ") + what + " needs 16-byte aligned size/offsets");
     if (nblocks < 1 || nblocks > kMaxCommBlocks) throw std::runtime_error("bagua: peer kernel grid must be 1.." + std::to_string(kMaxCommBlocks));
+    return bytes / 16;
 }
 }  // namespace
 
 void launch_allreduce(const PeerCtx& ctx, const PeerBuf& src, const PeerBuf& dst, size_t src_off, size_t dst_off,
                       size_t bytes, int dtype, float scale, int variant, int nblocks, int nthreads, cudaStream_t stream) {
-    if (bytes % 16 || src_off % 16 || dst_off % 16) throw std::runtime_error("bagua: allreduce needs 16-byte aligned size/offsets");
-    check_blocks(nblocks);
-    const size_t vecs = bytes / 16;
+    const size_t vecs = peer_vecs("allreduce", bytes, src_off, dst_off, nblocks);
     if (vecs == 0) return;
-    dispatch_float(dtype, [&](auto tag) {
+    dispatch_float(dtype, kFamily, [&](auto tag) {
         using T = decltype(tag);
         if (variant == AR_MULTIMEM) {
             if (!src.mc || !dst.mc) throw std::runtime_error("bagua: multimem allreduce requested but no multicast mapping");
             allreduce_multimem_kernel<T><<<nblocks, nthreads, 0, stream>>>(ctx, src, dst, src_off, dst_off, vecs, scale);
         } else {
             dispatch_world(ctx.world, [&](auto pw) {
-                constexpr int P = decltype(pw)::value;
-                allreduce_twoshot_kernel<T, P><<<nblocks, nthreads, 0, stream>>>(ctx, src, dst, src_off, dst_off, vecs, scale);
+                allreduce_twoshot_kernel<T, decltype(pw)::value><<<nblocks, nthreads, 0, stream>>>(ctx, src, dst, src_off, dst_off, vecs, scale);
             });
         }
     });
@@ -745,16 +562,12 @@ void launch_allreduce(const PeerCtx& ctx, const PeerBuf& src, const PeerBuf& dst
 
 void launch_allreduce_oneshot(const PeerCtx& ctx, const PeerBuf& staging, size_t staging_off, size_t slot_bytes, const void* in, void* out,
                               size_t bytes, int dtype, float scale, int nblocks, int nthreads, cudaStream_t stream, uint32_t call_parity) {
-    if (bytes % 16) throw std::runtime_error("bagua: one-shot allreduce needs a 16-byte multiple");
+    const size_t vecs = peer_vecs("one-shot allreduce", bytes, 0, 0, nblocks);
     if (bytes > slot_bytes) throw std::runtime_error("bagua: one-shot allreduce message larger than its staging slot");
-    check_blocks(nblocks);
-    const size_t vecs = bytes / 16;
     if (vecs == 0) return;
-    dispatch_float(dtype, [&](auto tag) {
-        using T = decltype(tag);
+    dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
-            constexpr int P = decltype(pw)::value;
-            allreduce_oneshot_kernel<T, P><<<nblocks, nthreads, 0, stream>>>(
+            allreduce_oneshot_kernel<decltype(tag), decltype(pw)::value><<<nblocks, nthreads, 0, stream>>>(
                 ctx, staging, staging_off, slot_bytes, static_cast<const char*>(in), static_cast<char*>(out), vecs, scale, call_parity);
         });
     });
@@ -764,20 +577,14 @@ void launch_allreduce_oneshot(const PeerCtx& ctx, const PeerBuf& staging, size_t
 void launch_allreduce_sgd(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off,
                           size_t bytes, int dtype, float* master, float* momentum, const SgdParams& hp, float scale,
                           bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream) {
-    if (bytes % 16 || g_off % 16 || w_off % 16) throw std::runtime_error("bagua: allreduce_sgd needs 16-byte aligned size/offsets");
-    check_blocks(nblocks);
-    const size_t vecs = bytes / 16;
+    const size_t vecs = peer_vecs("allreduce_sgd", bytes, g_off, w_off, nblocks);
     if (vecs == 0) return;
-    dispatch_float(dtype, [&](auto tag) {
-        using T = decltype(tag);
+    dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
-            constexpr int P = decltype(pw)::value;
-            if (use_multimem)
-                allreduce_sgd_kernel<T, P, true><<<nblocks, nthreads, 0, stream>>>(ctx, grads, weights, g_off, w_off, vecs, master,
-                                                                                 momentum, hp, scale, zero_grads ? 1 : 0);
-            else
-                allreduce_sgd_kernel<T, P, false><<<nblocks, nthreads, 0, stream>>>(ctx, grads, weights, g_off, w_off, vecs, master,
-                                                                                  momentum, hp, scale, zero_grads ? 1 : 0);
+            dispatch_mc(use_multimem, [&](auto mc) {
+                allreduce_sgd_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
+                    ctx, grads, weights, g_off, w_off, vecs, master, momentum, hp, scale, zero_grads ? 1 : 0);
+            });
         });
     });
     check_launch("allreduce_sgd");
@@ -785,18 +592,14 @@ void launch_allreduce_sgd(const PeerCtx& ctx, const PeerBuf& grads, const PeerBu
 
 void launch_reduce_scatter(const PeerCtx& ctx, const PeerBuf& buf, size_t off, size_t bytes, int dtype, float scale, bool use_multimem, int nblocks,
                            int nthreads, cudaStream_t stream) {
-    if (bytes % 16 || off % 16) throw std::runtime_error("bagua: reduce_scatter needs 16-byte aligned size/offset");
-    check_blocks(nblocks);
-    const size_t vecs = bytes / 16;
+    const size_t vecs = peer_vecs("reduce_scatter", bytes, off, 0, nblocks);
     if (vecs == 0) return;
-    dispatch_float(dtype, [&](auto tag) {
-        using T = decltype(tag);
+    dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
-            constexpr int P = decltype(pw)::value;
-            if (use_multimem)
-                reduce_scatter_kernel<T, P, true><<<nblocks, nthreads, 0, stream>>>(ctx, buf, off, vecs, scale);
-            else
-                reduce_scatter_kernel<T, P, false><<<nblocks, nthreads, 0, stream>>>(ctx, buf, off, vecs, scale);
+            dispatch_mc(use_multimem, [&](auto mc) {
+                reduce_scatter_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(ctx, buf, off, vecs,
+                                                                                                                               scale);
+            });
         });
     });
     check_launch("reduce_scatter");
@@ -804,18 +607,13 @@ void launch_reduce_scatter(const PeerCtx& ctx, const PeerBuf& buf, size_t off, s
 
 void launch_all_gather(const PeerCtx& ctx, const PeerBuf& buf, size_t off, size_t bytes, int dtype, bool use_multimem, int nblocks, int nthreads,
                        cudaStream_t stream) {
-    if (bytes % 16 || off % 16) throw std::runtime_error("bagua: all_gather needs 16-byte aligned size/offset");
-    check_blocks(nblocks);
-    const size_t vecs = bytes / 16;
+    const size_t vecs = peer_vecs("all_gather", bytes, off, 0, nblocks);
     if (vecs == 0) return;
-    dispatch_float(dtype, [&](auto tag) {
-        using T = decltype(tag);
+    dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
-            constexpr int P = decltype(pw)::value;
-            if (use_multimem)
-                all_gather_kernel<T, P, true><<<nblocks, nthreads, 0, stream>>>(ctx, buf, off, vecs);
-            else
-                all_gather_kernel<T, P, false><<<nblocks, nthreads, 0, stream>>>(ctx, buf, off, vecs);
+            dispatch_mc(use_multimem, [&](auto mc) {
+                all_gather_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(ctx, buf, off, vecs);
+            });
         });
     });
     check_launch("all_gather");
@@ -824,21 +622,15 @@ void launch_all_gather(const PeerCtx& ctx, const PeerBuf& buf, size_t off, size_
 void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
                            float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, float scale, bool zero_grads, bool use_multimem,
                            int nblocks, int nthreads, cudaStream_t stream) {
-    if (bytes % 16 || g_off % 16 || w_off % 16) throw std::runtime_error("bagua: allreduce_adam needs 16-byte aligned size/offsets");
+    const size_t vecs = peer_vecs("allreduce_adam", bytes, g_off, w_off, nblocks);
     if (hp.amsgrad) throw std::runtime_error("bagua: allreduce_adam does not implement amsgrad");
-    check_blocks(nblocks);
-    const size_t vecs = bytes / 16;
     if (vecs == 0) return;
-    dispatch_float(dtype, [&](auto tag) {
-        using T = decltype(tag);
+    dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
-            constexpr int P = decltype(pw)::value;
-            if (use_multimem)
-                allreduce_adam_kernel<T, P, true><<<nblocks, nthreads, 0, stream>>>(ctx, grads, weights, g_off, w_off, vecs, master, exp_avg,
-                                                                                  exp_avg_sq, hp, scale, zero_grads ? 1 : 0);
-            else
-                allreduce_adam_kernel<T, P, false><<<nblocks, nthreads, 0, stream>>>(ctx, grads, weights, g_off, w_off, vecs, master, exp_avg,
-                                                                                   exp_avg_sq, hp, scale, zero_grads ? 1 : 0);
+            dispatch_mc(use_multimem, [&](auto mc) {
+                allreduce_adam_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
+                    ctx, grads, weights, g_off, w_off, vecs, master, exp_avg, exp_avg_sq, hp, scale, zero_grads ? 1 : 0);
+            });
         });
     });
     check_launch("allreduce_adam");
@@ -846,13 +638,10 @@ void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerB
 
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,
                          int nblocks, int nthreads, cudaStream_t stream) {
-    if (bytes % 16 || off % 16) throw std::runtime_error("bagua: peer_average needs 16-byte aligned size/offset");
+    const size_t vecs = peer_vecs("peer_average", bytes, off, 0, nblocks);
     if (peer < 0 || peer >= ctx.world) throw std::runtime_error("bagua: peer_average peer rank out of range");
-    check_blocks(nblocks);
-    const size_t vecs = bytes / 16;
-    dispatch_float(dtype, [&](auto tag) {
-        using T = decltype(tag);
-        peer_average_kernel<T><<<nblocks, nthreads, 0, stream>>>(ctx, weights, off, peer, static_cast<char*>(out), vecs);
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        peer_average_kernel<decltype(tag)><<<nblocks, nthreads, 0, stream>>>(ctx, weights, off, peer, static_cast<char*>(out), vecs);
     });
     check_launch("peer_average");
 }
@@ -860,21 +649,15 @@ void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off,
 void launch_async_average(const PeerCtx& ctx, void* w, const PeerBuf& snap, size_t snap_off, const PeerBuf& avg, size_t avg_off, size_t bytes, int dtype,
                           uint32_t seq, bool go, uint32_t* gate, unsigned long long gate_timeout_ns, int* status, bool use_multimem, int nblocks, int nthreads,
                           cudaStream_t stream) {
-    if (bytes % 16 || snap_off % 16 || avg_off % 16) throw std::runtime_error("bagua: async_average needs 16-byte aligned size/offsets");
-    check_blocks(nblocks);
-    const size_t vecs = bytes / 16;
+    const size_t vecs = peer_vecs("async_average", bytes, snap_off, avg_off, nblocks);
     if (vecs == 0) return;
     if (use_multimem && (!snap.mc || !avg.mc)) throw std::runtime_error("bagua: multimem async_average requested but no multicast mapping");
-    dispatch_float(dtype, [&](auto tag) {
-        using T = decltype(tag);
+    dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
-            constexpr int P = decltype(pw)::value;
-            if (use_multimem)
-                async_average_kernel<T, P, true><<<nblocks, nthreads, 0, stream>>>(ctx, static_cast<char*>(w), snap, snap_off, avg, avg_off, vecs, seq, go ? 1 : 0,
-                                                                                 gate, gate_timeout_ns, status);
-            else
-                async_average_kernel<T, P, false><<<nblocks, nthreads, 0, stream>>>(ctx, static_cast<char*>(w), snap, snap_off, avg, avg_off, vecs, seq, go ? 1 : 0,
-                                                                                  gate, gate_timeout_ns, status);
+            dispatch_mc(use_multimem, [&](auto mc) {
+                async_average_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
+                    ctx, static_cast<char*>(w), snap, snap_off, avg, avg_off, vecs, seq, go ? 1 : 0, gate, gate_timeout_ns, status);
+            });
         });
     });
     check_launch("async_average");

@@ -3,7 +3,7 @@
 reduces the slots it received.  Calls use different grid sizes (1-8 CTAs by message size, ``PeerEngine.launch_cfg``).
 
 The round-1 kernel took the parity from the per-CTA epoch; CTAs that sit out small calls then fall out of step with CTA 0 and a
-fast rank can overwrite a slot a slow peer is still reading (ADVICE.md, peer_kernels.cu:210).  The fix takes the parity from a
+fast rank can overwrite a slot a slow peer is still reading (ADVICE.md; the comment on ``parity`` in ``allreduce_oneshot_kernel``).  The fix takes the parity from a
 per-communicator CALL counter kept by the host (``PeerComm::next_oneshot_parity``).  The model executes random interleavings of the
 CTAs of 2-3 ranks over random call sequences, with per-rank stream order (kernel c+1 starts when kernel c has retired) and the
 real barrier rule (row b waits for row b of every peer), and checks every read: each slot must hold exactly the data of THIS call.

@@ -36,8 +36,27 @@ def _code(dtype):
     return dtype_code(dtype)
 
 
-def _tol(dtype):
-    return {torch.float32: 1e-5, torch.bfloat16: 2e-2, torch.float16: 3e-3}[dtype]
+def _f32(x):
+    return torch.tensor(x, dtype=torch.float32)
+
+
+def _owned_slice_sum(xs, scale):
+    """Bit-exact oracle of the owned-slice reduction (fp32, on the CPU): the vectors of slice s start from rank s's copy, add rank
+    (s + i) % P for i = 1 .. P-1 in that order, and are multiplied by the fp32 ``scale``.  Rounding to the dtype is the caller's."""
+    P, numel = len(xs), xs[0].numel()
+    per = 16 // xs[0].element_size()
+    vpr = (numel // per + P - 1) // P
+    xs = [x.cpu().float() for x in xs]
+    out = torch.empty(numel, dtype=torch.float32)
+    for s in range(P):
+        lo, hi = s * vpr * per, min((s + 1) * vpr * per, numel)
+        if lo >= hi:
+            continue
+        acc = xs[s][lo:hi].clone()
+        for i in range(1, P):
+            acc += xs[(s + i) % P][lo:hi]
+        out[lo:hi] = acc * scale
+    return out
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -56,18 +75,16 @@ def test_twoshot_allreduce_matches_fp32_sum(C, P, dtype):
         dst = w.alloc(nbytes)
         for r in range(P):
             src.view(r, dtype, numel).copy_(xs[r])
-        ref = sum(x.float() for x in xs) / P
+        ref = _owned_slice_sum(xs, _f32(1.0 / P)).to(dtype)
         # out of place, then in place (twice: epochs advance, no reset)
         w.run(lambda r: C.AllReduceOp(w.comms[r], src.buf, dst.buf, 0, 0, nbytes, _code(dtype), 1.0 / P, C.AR_TWO_SHOT, w.cfg(4)))
         for r in range(P):
-            err = (dst.view(r, dtype, numel).float() - ref).abs().max().item()
-            assert err <= _tol(dtype) * max(1.0, ref.abs().max().item()), (P, dtype, numel, r, err)
+            assert torch.equal(dst.view(r, dtype, numel).cpu(), ref), (P, dtype, numel, r)
             assert torch.equal(src.view(r, dtype, numel), xs[r])   # source untouched
         w.run(lambda r: C.AllReduceOp(w.comms[r], src.buf, src.buf, 0, 0, nbytes, _code(dtype), 1.0, C.AR_TWO_SHOT, w.cfg(7)))
-        ref_sum = sum(x.float() for x in xs)
+        ref_sum = _owned_slice_sum(xs, _f32(1.0)).to(dtype)
         for r in range(P):
-            err = (src.view(r, dtype, numel).float() - ref_sum).abs().max().item()
-            assert err <= _tol(dtype) * max(1.0, ref_sum.abs().max().item()) * P, (P, dtype, numel, r, err)
+            assert torch.equal(src.view(r, dtype, numel).cpu(), ref_sum), (P, dtype, numel, r)
 
 
 @pytest.mark.parametrize("P", WORLDS)
@@ -87,9 +104,12 @@ def test_oneshot_allreduce_parity_survives_mixed_grids(C, P):
         ops = [C.AllReduceOneShotOp(w.comms[r], staging.buf, 0, ONE_SHOT_SLOT, xs[r].data_ptr(), outs[r].data_ptr(), nbytes, _code(dtype), 1.0 / P, w.cfg(blocks))
                for r in range(P)]
         w.run(None, ops=ops)
-        ref = sum(xs) / P
+        ref = xs[0].cpu().clone()   # every rank sums the staging slots in slot order 0 .. P-1
+        for p in range(1, P):
+            ref += xs[p].cpu()
+        ref = ref * _f32(1.0 / P)
         for r in range(P):
-            torch.testing.assert_close(outs[r], ref, rtol=1e-5, atol=1e-5)
+            assert torch.equal(outs[r].cpu(), ref), (P, i, r)
 
 
 @pytest.mark.parametrize("P", [2, 4, 8])
@@ -105,17 +125,16 @@ def test_reduce_scatter_then_all_gather(C, P, dtype):
     for r in range(P):
         buf.view(r, dtype, numel).copy_(xs[r])
     w.run(lambda r: C.ReduceScatterOp(w.comms[r], buf.buf, 0, nbytes, _code(dtype), 1.0 / P, False, w.cfg(4)))
-    ref = sum(x.float() for x in xs) / P
+    ref = _owned_slice_sum(xs, _f32(1.0 / P)).to(dtype)
     per = 16 // es
     vecs = nbytes // 16
     vpr = (vecs + P - 1) // P
     for r in range(P):
         lo, hi = r * vpr * per, min((r + 1) * vpr * per, numel)
-        got = buf.view(r, dtype, numel)[lo:hi].float()
-        assert (got - ref[lo:hi]).abs().max().item() <= _tol(dtype) * max(1.0, ref.abs().max().item())
+        assert torch.equal(buf.view(r, dtype, numel)[lo:hi].cpu(), ref[lo:hi]), (P, dtype, r)
     w.run(lambda r: C.AllGatherOp(w.comms[r], buf.buf, 0, nbytes, _code(dtype), False, w.cfg(4)))
     for r in range(P):
-        assert (buf.view(r, dtype, numel).float() - ref).abs().max().item() <= _tol(dtype) * max(1.0, ref.abs().max().item())
+        assert torch.equal(buf.view(r, dtype, numel).cpu(), ref), (P, dtype, r)
     for r in range(1, P):
         assert torch.equal(buf.view(r, dtype, numel), buf.view(0, dtype, numel))   # bit-identical replicas
 
@@ -232,7 +251,7 @@ def test_peer_average_shift_one_pairs_and_values(C, P):
         for r in range(P):
             peer = C.PeerAverageOp.shift_one_peer(r, P, step)
             assert C.PeerAverageOp.shift_one_peer(peer, P, step) == r, "pairing must be symmetric"
-            torch.testing.assert_close(outs[r], (xs[r] + xs[peer]) / 2, rtol=1e-6, atol=1e-6)
+            assert torch.equal(outs[r].cpu(), (xs[r].cpu() + xs[peer].cpu()) * _f32(0.5)), (P, step, r)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -373,12 +392,13 @@ def test_async_average_kernel_round_and_abort_vote(C, P, dtype):
     ops = [C.AsyncAverageOp(w.comms[r], weights[r].data_ptr(), snap.buf, 0, avg.buf, 0, nbytes, _code(dtype), gates[r], 2.0, False, w.cfg(5)) for r in range(P)]
     x0 = [x.clone() for x in weights]
     w.run(None, ops=ops)
-    mean = sum(x.float() for x in x0) / P
+    # the mean is rounded to the dtype when it is published; then w += mean - snapshot in fp32, with snapshot == w here
+    mean = _owned_slice_sum(x0, _f32(1.0) / P).to(dtype).float()
+    want = [(x.cpu().float() + (mean - x.cpu().float())).to(dtype) for x in x0]
     for r in range(P):
         assert ops[r].status() == 1
         assert gates[r].state() == 0, "the gate must be handed back"
-        # w += mean - snapshot with snapshot == w: the result is the mean (rounded through the dtype twice)
-        assert (weights[r].float() - mean).abs().max().item() <= 2 * _tol(dtype) * max(1.0, mean.abs().max().item())
+        assert torch.equal(weights[r].cpu(), want[r]), (P, dtype, r)
     # second round with the trainer holding the gate on rank 0: that rank skips the apply after the bounded wait, the others average
     if P > 1:
         ops2 = [C.AsyncAverageOp(w.comms[r], weights[r].data_ptr(), snap.buf, 0, avg.buf, 0, nbytes, _code(dtype), gates[r], 0.2, False, w.cfg(5)) for r in range(P)]
@@ -389,7 +409,7 @@ def test_async_average_kernel_round_and_abort_vote(C, P, dtype):
         assert gates[0].state() == 1
         w.run(None, ops=ops2)
         assert torch.equal(weights[0], x0[0]), "weights must not change while the trainer holds the gate"
-        assert (weights[1].float() - mean).abs().max().item() <= 2 * _tol(dtype) * max(1.0, mean.abs().max().item())
+        assert torch.equal(weights[1].cpu(), want[1])
         gates[0].release(torch.cuda.current_stream().cuda_stream)
         torch.cuda.synchronize()
         assert gates[0].state() == 0
@@ -407,7 +427,7 @@ def test_async_average_kernel_round_and_abort_vote(C, P, dtype):
     w.run(None, ops=ops)
     for r in range(P):
         assert ops[r].status() == 1
-        assert (weights[r].float() - mean).abs().max().item() <= 2 * _tol(dtype) * max(1.0, mean.abs().max().item())
+        assert torch.equal(weights[r].cpu(), want[r]), (P, dtype, r)
 
 
 def test_weight_gate_orders_apply_after_the_trainer_release(C):
