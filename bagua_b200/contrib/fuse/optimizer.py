@@ -119,7 +119,7 @@ def _kernel_kind(optimizer) -> Optional[str]:
 def _kernel_step(opt, kind: str) -> bool:
     """Run one step of SGD/Adam/AdamW through the multi-tensor kernels; returns False if a group is not eligible."""
     from ...core import dtype_code, native
-    from ...ops.optim import _MultiPlan
+    from ...ops.optim import _cached_plan, _launch_groups
 
     C = native()
     plans = opt.__dict__.setdefault("_bagua_kernel_plans", {})
@@ -137,13 +137,21 @@ def _kernel_step(opt, kind: str) -> bool:
     stream = torch.cuda.current_stream().cuda_stream
     for gi, group in enumerate(opt.param_groups):
         params = [p for p in group["params"] if p.grad is not None]
-        by_dtype: Dict[torch.dtype, List[torch.nn.Parameter]] = {}
-        for p in params:
-            by_dtype.setdefault(p.dtype, []).append(p)
-        for dt, ps in by_dtype.items():
+        if kind == "sgd":
+            mom = group["momentum"]
+            groups = _launch_groups(params, lambda p: mom != 0 and opt.state[p].get("momentum_buffer") is not None)
+        else:
+            for p in params:
+                st = opt.state[p]
+                if len(st) == 0:
+                    st["step"] = torch.tensor(0.0)
+                    st["exp_avg"] = torch.zeros_like(p.data)
+                    st["exp_avg_sq"] = torch.zeros_like(p.data)
+                st["step"] = st["step"] + 1
+            groups = _launch_groups(params, lambda p: int(opt.state[p]["step"]))
+        for (dt, k), ps in groups:
             if kind == "sgd":
-                mom = group["momentum"]
-                first = mom != 0 and any("momentum_buffer" not in opt.state[p] or opt.state[p]["momentum_buffer"] is None for p in ps)
+                first = mom != 0 and opt.state[ps[0]].get("momentum_buffer") is None
                 lists = [[p.data for p in ps], [p.grad for p in ps]]
                 if mom != 0:
                     for p in ps:
@@ -151,20 +159,9 @@ def _kernel_step(opt, kind: str) -> bool:
                             opt.state[p]["momentum_buffer"] = torch.zeros_like(p.data)
                     lists.append([opt.state[p]["momentum_buffer"] for p in ps])
             else:
-                for p in ps:
-                    st = opt.state[p]
-                    if len(st) == 0:
-                        st["step"] = torch.tensor(0.0)
-                        st["exp_avg"] = torch.zeros_like(p.data)
-                        st["exp_avg_sq"] = torch.zeros_like(p.data)
-                    st["step"] = st["step"] + 1 if isinstance(st["step"], torch.Tensor) else st["step"] + 1
                 step = int(opt.state[ps[0]]["step"])
                 lists = [[p.data for p in ps], [p.grad for p in ps], [opt.state[p]["exp_avg"] for p in ps], [opt.state[p]["exp_avg_sq"] for p in ps]]
-            sig = tuple(t.data_ptr() for lst in lists for t in lst)
-            plan = plans.get((gi, dt))
-            if plan is None or plan.signature != sig:
-                plan = _MultiPlan(lists)
-                plans[(gi, dt)] = plan
+            plan = _cached_plan(plans, (gi, dt, k), lists)
             if kind == "sgd":
                 C.multi_tensor_sgd(*plan.args(), dtype_code(dt), mom != 0, float(group["lr"]), float(mom), float(group["dampening"]),
                                    float(group["weight_decay"]), bool(group["nesterov"]), bool(first), 1.0, stream)

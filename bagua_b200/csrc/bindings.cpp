@@ -312,6 +312,13 @@ PYBIND11_MODULE(_C, m) {
                                reinterpret_cast<const int32_t*>(b2t), reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk};
               launch_multi_tensor_sgd(d, dtype, has_mom, make_sgd(lr, momentum, dampening, wd, nesterov, first_step), grad_scale, S(stream));
           });
+    m.def("multi_tensor_sgd_mp",
+          [](uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, int dtype, bool has_mom,
+             float lr, float momentum, float dampening, float wd, bool nesterov, bool first_step, float grad_scale, uint64_t stream) {
+              TensorListDesc d{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes),
+                               reinterpret_cast<const int32_t*>(b2t), reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk};
+              launch_multi_tensor_sgd_mp(d, dtype, has_mom, make_sgd(lr, momentum, dampening, wd, nesterov, first_step), grad_scale, S(stream));
+          });
     m.def("multi_tensor_adam",
           [](uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, int dtype, float lr, float b1,
              float b2, float eps, float wd, int step, bool adamw, float grad_scale, uint64_t stream) {

@@ -172,6 +172,9 @@ void launch_multi_tensor_sgd(const TensorListDesc& d, int dtype, bool has_moment
 void launch_multi_tensor_adam(const TensorListDesc& d, int dtype, const AdamParams& hp, float grad_scale, cudaStream_t stream);
 // mixed precision: lists [param(T), grad(T), exp_avg(f32), exp_avg_sq(f32), master(f32)]
 void launch_multi_tensor_adam_mp(const TensorListDesc& d, int dtype, const AdamParams& hp, float grad_scale, cudaStream_t stream);
+// mixed precision: lists [param(T), grad(T), master(f32)(, momentum(f32) when has_momentum)]
+void launch_multi_tensor_sgd_mp(const TensorListDesc& d, int dtype, bool has_momentum, const SgdParams& hp, float grad_scale,
+                                cudaStream_t stream);
 // QAdam momentum pre-step (bagua/torch_api/algorithms/q_adam.py:193-221): m = beta1*m + (1-beta1)*g
 void launch_qadam_momentum(float* exp_avg, const void* grad, int grad_dtype, size_t numel, float beta1, cudaStream_t stream);
 

@@ -282,6 +282,40 @@ __global__ void __launch_bounds__(kThreads) multi_tensor_adam_mp_kernel(TensorLi
     }
 }
 
+// Mixed precision: lists = [param(T), grad(T), master(f32)(, momentum(f32))] — the SGD counterpart of the kernel above.
+template <typename T, bool HAS_MOM>
+__global__ void __launch_bounds__(kThreads) multi_tensor_sgd_mp_kernel(TensorListDesc d, SgdParams hp, float grad_scale) {
+    const int t = d.block_to_tensor[blockIdx.x];
+    const size_t off = static_cast<size_t>(d.block_to_chunk[blockIdx.x]) * d.chunk;
+    const size_t n = static_cast<size_t>(d.sizes[t]);
+    const size_t len = (n - off) < static_cast<size_t>(d.chunk) ? (n - off) : static_cast<size_t>(d.chunk);
+    T* p = reinterpret_cast<T*>(d.ptrs[t]) + off;
+    const T* g = reinterpret_cast<const T*>(d.ptrs[d.n_tensors + t]) + off;
+    float* mw = reinterpret_cast<float*>(d.ptrs[2 * d.n_tensors + t]) + off;
+    float* mo = HAS_MOM ? reinterpret_cast<float*>(d.ptrs[3 * d.n_tensors + t]) + off : nullptr;
+    for (size_t i = threadIdx.x; i < len; i += blockDim.x) {
+        float w = mw[i];
+        float m = (HAS_MOM && !hp.first_step) ? mo[i] : 0.f;
+        sgd_update(w, to_f32<T>(g[i]), m, hp, grad_scale);
+        mw[i] = w;
+        if (HAS_MOM) mo[i] = m;
+        p[i] = from_f32<T>(w);
+    }
+}
+
+void launch_multi_tensor_sgd_mp(const TensorListDesc& d, int dtype, bool has_momentum, const SgdParams& hp, float grad_scale,
+                                cudaStream_t stream) {
+    if (d.n_blocks <= 0) return;
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
+        using T = decltype(tag);
+        if (has_momentum)
+            multi_tensor_sgd_mp_kernel<T, true><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, grad_scale);
+        else
+            multi_tensor_sgd_mp_kernel<T, false><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, grad_scale);
+    });
+    check_launch("multi_tensor_sgd_mp");
+}
+
 void launch_multi_tensor_adam_mp(const TensorListDesc& d, int dtype, const AdamParams& hp, float grad_scale, cudaStream_t stream) {
     if (d.n_blocks <= 0) return;
     dispatch_float(dtype, "optimizer kernels", [&](auto tag) {

@@ -82,6 +82,37 @@ def multi_tensor_plan(lists: List[List[torch.Tensor]]) -> _MultiPlan:
     return _MultiPlan(lists)
 
 
+def _launch_groups(params, state_key) -> List[tuple]:
+    """Split ``params`` into multi-tensor launches: one per (dtype, ``state_key(p)``), in order of first appearance.  One launch
+    applies one set of scalars (first step, bias correction) to all its tensors, so parameters whose optimizer state differs —
+    one whose gradient was ``None`` at earlier steps — must not share it.  Returns ``[((dtype, ordinal), params)]``; the ordinal
+    counts the launches of that dtype, so the pair stays the same from step to step and keys the plan cache."""
+    groups: Dict[tuple, List[torch.nn.Parameter]] = {}
+    for p in params:
+        groups.setdefault((p.dtype, state_key(p)), []).append(p)
+    out, seen = [], {}
+    for (dt, _), ps in groups.items():
+        seen[dt] = seen.get(dt, -1) + 1
+        out.append(((dt, seen[dt]), ps))
+    return out
+
+
+def _cached_plan(cache: dict, key, lists: List[List[torch.Tensor]]) -> _MultiPlan:
+    plan = cache.get(key)
+    if plan is None or plan.signature != tuple(t.data_ptr() for lst in lists for t in lst):
+        plan = cache[key] = _MultiPlan(lists)
+    return plan
+
+
+def _grad_in_layout(p: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """``p.grad`` in ``dtype`` and in ``p``'s memory layout: the multi-tensor kernels address parameter, gradient and state
+    with one flat index over raw memory (a channels_last parameter may well receive a contiguous gradient)."""
+    g = p.grad
+    if g.dtype == dtype and g.stride() == p.stride():
+        return g
+    return torch.empty_like(p.data, dtype=dtype).copy_(g)
+
+
 class _Segment:
     """A span of the gradient arena owned by one param group: grads, params and state share flat indices."""
 
@@ -190,7 +221,7 @@ class _FusedBase(torch.optim.Optimizer):
         self.master_weights = master_weights
         self.zero_grad_in_step = zero_grad_in_step
         self._segments: Dict[int, Optional[_Segment]] = {}
-        self._multi: Dict[int, _MultiPlan] = {}
+        self._multi: Dict[tuple, _MultiPlan] = {}
         self._grads_zeroed = False
         self.kernel_launches = 0
 
@@ -353,25 +384,30 @@ class FusedSGD(_FusedBase):
             if not _kernels_apply(params):
                 self._torch_step(params, group)
                 continue
-            by_dtype: Dict[torch.dtype, List[torch.nn.Parameter]] = {}
-            for p in params:
-                by_dtype.setdefault(p.dtype, []).append(p)
-            for dt, ps in by_dtype.items():
-                first = "momentum_buffer" not in self.state[ps[0]]
-                lists = [[p.data for p in ps], [p.grad.to(dt) if p.grad.dtype != dt else p.grad for p in ps]]
+            for (dt, k), ps in _launch_groups(params, lambda p: mom != 0 and "momentum_buffer" in self.state[p]):
+                # low-precision parameters keep fp32 master weights and fp32 momentum (mixed-precision kernel)
+                mixed = self.master_weights and dt in (torch.float16, torch.bfloat16)
+                first = mom != 0 and "momentum_buffer" not in self.state[ps[0]]
+                for p in ps:
+                    st = self.state[p]
+                    if mixed and "master" not in st:
+                        st["master"] = torch.empty_like(p.data, dtype=torch.float32).copy_(p.data)
+                    if mom != 0:
+                        sdt = torch.float32 if mixed else p.dtype
+                        buf = st.get("momentum_buffer")
+                        if buf is None:
+                            st["momentum_buffer"] = torch.zeros_like(p.data, dtype=sdt)
+                        elif buf.dtype != sdt or buf.stride() != p.stride():  # e.g. a checkpoint written with another precision
+                            st["momentum_buffer"] = torch.empty_like(p.data, dtype=sdt).copy_(buf)
+                lists = [[p.data for p in ps], [_grad_in_layout(p, dt) for p in ps]]
+                if mixed:
+                    lists.append([self.state[p]["master"] for p in ps])
                 if mom != 0:
-                    for p in ps:
-                        if "momentum_buffer" not in self.state[p]:
-                            self.state[p]["momentum_buffer"] = torch.zeros_like(p.data)
                     lists.append([self.state[p]["momentum_buffer"] for p in ps])
-                key = (gi, dt)
-                plan = self._multi.get(key)
-                sig = tuple(t.data_ptr() for lst in lists for t in lst)
-                if plan is None or plan.signature != sig:
-                    plan = _MultiPlan(lists)
-                    self._multi[key] = plan
-                C.multi_tensor_sgd(*plan.args(), dtype_code(dt), mom != 0, float(lr), float(mom), float(damp), float(wd), bool(nest), bool(first),
-                                   float(self.grad_scale), _stream())
+                plan = _cached_plan(self._multi, (gi, dt, k), lists)
+                fn = C.multi_tensor_sgd_mp if mixed else C.multi_tensor_sgd
+                fn(*plan.args(), dtype_code(dt), mom != 0, float(lr), float(mom), float(damp), float(wd), bool(nest), bool(first),
+                   float(self.grad_scale), _stream())
                 self.kernel_launches += 1
         if only is None:
             self._grads_zeroed = self.zero_grad_in_step and all(s is not None for s in self._segments.values()) and len(self._segments) == len(self.param_groups)
@@ -435,33 +471,27 @@ class FusedAdam(_FusedBase):
             if not _kernels_apply(params):
                 self._torch_step(params, group)
                 continue
-            by_dtype: Dict[torch.dtype, List[torch.nn.Parameter]] = {}
             for p in params:
-                by_dtype.setdefault(p.dtype, []).append(p)
-            for dt, ps in by_dtype.items():
-                # low-precision parameters keep fp32 moments and fp32 master weights (mixed-precision kernel)
+                st = self.state[p]
+                if "exp_avg" not in st:
+                    # low-precision parameters keep fp32 moments and fp32 master weights (mixed-precision kernel)
+                    mixed = self.master_weights and p.dtype in (torch.float16, torch.bfloat16)
+                    sdt = torch.float32 if mixed else p.dtype
+                    # preserve_format: state shares the parameter's memory order (the kernel walks raw memory)
+                    st["exp_avg"] = torch.zeros_like(p.data, dtype=sdt)
+                    st["exp_avg_sq"] = torch.zeros_like(p.data, dtype=sdt)
+                    st["step"] = 0
+                    if mixed:
+                        st["master"] = torch.empty_like(p.data, dtype=torch.float32).copy_(p.data)
+                st["step"] += 1
+            for (dt, k), ps in _launch_groups(params, lambda p: int(self.state[p]["step"])):
                 mixed = self.master_weights and dt in (torch.float16, torch.bfloat16)
-                for p in ps:
-                    st = self.state[p]
-                    if "exp_avg" not in st:
-                        sdt = torch.float32 if mixed else p.dtype
-                        # preserve_format: state shares the parameter's memory order (the kernel walks raw memory)
-                        st["exp_avg"] = torch.zeros_like(p.data, dtype=sdt)
-                        st["exp_avg_sq"] = torch.zeros_like(p.data, dtype=sdt)
-                        st["step"] = 0
-                        if mixed:
-                            st["master"] = torch.empty_like(p.data, dtype=torch.float32).copy_(p.data)
-                    st["step"] += 1
-                step = self.state[ps[0]]["step"]
-                lists = [[p.data for p in ps], [p.grad for p in ps], [self.state[p]["exp_avg"] for p in ps], [self.state[p]["exp_avg_sq"] for p in ps]]
+                step = int(self.state[ps[0]]["step"])
+                lists = [[p.data for p in ps], [_grad_in_layout(p, dt) for p in ps], [self.state[p]["exp_avg"] for p in ps],
+                         [self.state[p]["exp_avg_sq"] for p in ps]]
                 if mixed:
                     lists.append([self.state[p]["master"] for p in ps])
-                key = (gi, dt)
-                plan = self._multi.get(key)
-                sig = tuple(t.data_ptr() for lst in lists for t in lst)
-                if plan is None or plan.signature != sig:
-                    plan = _MultiPlan(lists)
-                    self._multi[key] = plan
+                plan = _cached_plan(self._multi, (gi, dt, k), lists)
                 fn = C.multi_tensor_adam_mp if mixed else C.multi_tensor_adam
                 fn(*plan.args(), dtype_code(dt), float(lr), float(betas[0]), float(betas[1]), float(eps), float(wd), int(step), bool(adamw),
                    float(self.grad_scale), _stream())

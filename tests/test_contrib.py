@@ -460,28 +460,32 @@ def test_python_nhwc_functions_finish_path_with_the_host_double(tmp_path, monkey
     nhwc._workspaces.clear()
 
 
+def _np_view(ptr, n, np_dtype):
+    """numpy array over ``n`` elements of host memory at address ``ptr``."""
+    import ctypes
+
+    return np.ctypeslib.as_array((ctypes.c_uint8 * (n * np.dtype(np_dtype).itemsize)).from_address(ptr)).view(np_dtype)
+
+
+def _bf16_to_f32(u16):
+    return (u16.astype(np.uint32) << 16).view(np.float32)
+
+
+def _f32_to_bf16(f):
+    u = f.astype(np.float32).view(np.uint32)
+    return ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
+
+
 def test_fused_adam_multi_tensor_call_sites_with_a_numpy_kernel_double(monkeypatch):
     """FusedAdam's multi-tensor path (parameters outside the bucket arena) on CPU: the pointer tables built by ``_MultiPlan`` are
     decoded by a numpy stand-in of ``multi_tensor_adam`` / ``multi_tensor_adam_mp`` that applies the Adam update in place — checks the
     list order [param, grad, exp_avg, exp_avg_sq(, master)], the fp32 state of bf16 parameters and the chunk/block map against
     ``torch.optim.AdamW``."""
-    import ctypes
     import types
-
-    import numpy as np
 
     from bagua_b200.ops import optim
 
-    def view(ptr, n, np_dtype):
-        return np.ctypeslib.as_array((ctypes.c_uint8 * (n * np.dtype(np_dtype).itemsize)).from_address(ptr)).view(np_dtype)
-
-    def bf16_to_f32(u16):
-        return (u16.astype(np.uint32) << 16).view(np.float32)
-
-    def f32_to_bf16(f):
-        u = f.astype(np.float32).view(np.uint32)
-        return ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
-
+    view, bf16_to_f32, f32_to_bf16 = _np_view, _bf16_to_f32, _f32_to_bf16
     calls = {"mp": 0, "plain": 0}
 
     def adam(ptrs, sizes, b2t, b2c, n_t, n_blocks, chunk, dtype, lr, b1, b2, eps, wd, step, adamw, grad_scale, stream, mixed):
@@ -542,6 +546,129 @@ def test_fused_adam_multi_tensor_call_sites_with_a_numpy_kernel_double(monkeypat
                 assert "master" not in st
                 torch.testing.assert_close(p.data, r.data, rtol=1e-4, atol=1e-5)
     assert calls == {"mp": 6, "plain": 6}
+
+
+def _numpy_multi_tensor_kernels(launches):
+    """Host doubles of ``multi_tensor_sgd[_mp]`` / ``multi_tensor_adam[_mp]`` (fp32 and bf16 tensors): decode the ``_MultiPlan``
+    tables and apply the update in place, appending ``(kernel, first_step or step, n_tensors)`` to ``launches``."""
+    import types
+
+    def tensors(ptrs, sizes, b2t, b2c, n_t, n_blocks, chunk, n_lists):
+        P, S = _np_view(ptrs, n_lists * n_t, np.int64), _np_view(sizes, n_t, np.int64)
+        T, Ck = _np_view(b2t, n_blocks, np.int32), _np_view(b2c, n_blocks, np.int32)
+        for blk in range(n_blocks):
+            t, off = int(T[blk]), int(Ck[blk]) * chunk
+            n = min(int(S[t]) - off, chunk)
+            yield [(lambda base: (lambda np_dt: _np_view(int(base), int(S[t]), np_dt)[off:off + n]))(P[k * n_t + t]) for k in range(n_lists)]
+
+    def load(raw, dtype):
+        return _bf16_to_f32(raw(np.uint16)) if dtype == 4 else raw(np.float32).copy()
+
+    def store(raw, dtype, f):
+        if dtype == 4:
+            raw(np.uint16)[:] = _f32_to_bf16(f)
+        else:
+            raw(np.float32)[:] = f
+
+    def sgd(*a, mp):
+        ptrs, sizes, b2t, b2c, n_t, n_blocks, chunk, dtype, has_mom, lr, mom, damp, wd, nest, first, scale, _ = a
+        f32 = np.float32
+        for lists in tensors(ptrs, sizes, b2t, b2c, n_t, n_blocks, chunk, 2 + int(mp) + int(has_mom)):
+            w = load(lists[2], 0) if mp else load(lists[0], dtype)
+            d = load(lists[1], dtype) * f32(scale) + f32(wd) * w
+            if has_mom:
+                mdt = 0 if mp else dtype
+                m = d if first else f32(mom) * load(lists[-1], mdt) + f32(1 - damp) * d
+                store(lists[-1], mdt, m)
+                d = d + f32(mom) * m if nest else m
+            w = w - f32(lr) * d
+            if mp:
+                store(lists[2], 0, w)
+            store(lists[0], dtype, w)
+        launches.append(("sgd_mp" if mp else "sgd", bool(first), n_t))
+
+    def adam(*a, mp):
+        ptrs, sizes, b2t, b2c, n_t, n_blocks, chunk, dtype, lr, b1, b2, eps, wd, step, adamw, scale, _ = a
+        sdt = 0 if mp else dtype
+        for lists in tensors(ptrs, sizes, b2t, b2c, n_t, n_blocks, chunk, 5 if mp else 4):
+            w = load(lists[4], 0) if mp else load(lists[0], dtype)
+            g = load(lists[1], dtype) * scale
+            if adamw:
+                w = w * (1 - lr * wd)
+            else:
+                g = g + wd * w
+            m1 = b1 * load(lists[2], sdt) + (1 - b1) * g
+            m2 = b2 * load(lists[3], sdt) + (1 - b2) * g * g
+            w = w - (lr / (1 - b1 ** step)) * (m1 / (np.sqrt(m2) / np.sqrt(1 - b2 ** step) + eps))
+            store(lists[2], sdt, m1)
+            store(lists[3], sdt, m2)
+            if mp:
+                store(lists[4], 0, w)
+            store(lists[0], dtype, w)
+        launches.append(("adam_mp" if mp else "adam", int(step), n_t))
+
+    return types.SimpleNamespace(multi_tensor_sgd=lambda *a: sgd(*a, mp=False), multi_tensor_sgd_mp=lambda *a: sgd(*a, mp=True),
+                                 multi_tensor_adam=lambda *a: adam(*a, mp=False), multi_tensor_adam_mp=lambda *a: adam(*a, mp=True))
+
+
+@pytest.mark.parametrize("late", [0, 2], ids=["first", "last"])
+@pytest.mark.parametrize("kind", ["sgd", "adam"])
+def test_fused_optimizers_keep_per_parameter_state_when_a_parameter_joins_late(monkeypatch, kind, late):
+    """FusedSGD / FusedAdam on their multi-tensor path with numpy doubles of the kernels: a parameter whose gradient is None for the
+    first two steps starts with a first step of its own (momentum = d, bias correction of step 1), and the other parameters keep
+    their momentum and step counts — as in torch.optim.  Launches are split by state; once the state agrees again (Adam never, SGD
+    after the late parameter's first step) one launch per dtype remains."""
+    from bagua_b200.ops import optim
+
+    launches = []
+    monkeypatch.setattr(optim, "native", lambda: _numpy_multi_tensor_kernels(launches))
+    monkeypatch.setattr(optim, "_kernels_apply", lambda params: True)
+    monkeypatch.setattr(optim, "_stream", lambda: 0)
+    monkeypatch.setattr(optim._MultiPlan, "CHUNK", 1000)
+    torch.manual_seed(10)
+    ps = [torch.nn.Parameter(torch.randn(s)) for s in [(1500,), (7, 3), (33,)]]
+    rs = [torch.nn.Parameter(p.detach().clone()) for p in ps]
+    if kind == "sgd":
+        opt, ropt = optim.FusedSGD(ps, lr=0.1, momentum=0.9, dampening=0.25), torch.optim.SGD(rs, lr=0.1, momentum=0.9, dampening=0.25)
+    else:
+        opt, ropt = optim.FusedAdam(ps, lr=1e-2), torch.optim.Adam(rs, lr=1e-2)
+    for step in range(5):
+        for i, (p, r) in enumerate(zip(ps, rs)):
+            g = None if (i == late and step < 2) else torch.randn_like(p)
+            p.grad, r.grad = g, g
+        opt.step()
+        ropt.step()
+        for p, r in zip(ps, rs):
+            torch.testing.assert_close(p.data, r.data, rtol=1e-5, atol=1e-6)
+    # (first step or step count, tensors) of every launch; the late parameter's launch comes first when it is listed first
+    expected = {
+        ("sgd", 0): [(True, 2), (False, 2), (True, 1), (False, 2), (False, 3), (False, 3)],
+        ("sgd", 2): [(True, 2), (False, 2), (False, 2), (True, 1), (False, 3), (False, 3)],
+        ("adam", 0): [(1, 2), (2, 2), (1, 1), (3, 2), (2, 1), (4, 2), (3, 1), (5, 2)],
+        ("adam", 2): [(1, 2), (2, 2), (3, 2), (1, 1), (4, 2), (2, 1), (5, 2), (3, 1)],
+    }[(kind, late)]
+    assert [(s, n) for _, s, n in launches] == expected
+
+
+def test_fused_sgd_keeps_fp32_master_weights_for_bf16_parameters_off_the_flat_path(monkeypatch):
+    """A bf16 parameter outside any bucket: FusedSGD(master_weights=True) keeps fp32 ``master`` and ``momentum_buffer`` and
+    accumulates updates far below half a bf16 ulp of the weights in the master."""
+    from bagua_b200.ops import optim
+
+    launches = []
+    monkeypatch.setattr(optim, "native", lambda: _numpy_multi_tensor_kernels(launches))
+    monkeypatch.setattr(optim, "_kernels_apply", lambda params: True)
+    monkeypatch.setattr(optim, "_stream", lambda: 0)
+    p, q = torch.nn.Parameter(torch.ones(300, dtype=torch.bfloat16)), torch.nn.Parameter(torch.ones(7, dtype=torch.bfloat16))
+    opt = optim.FusedSGD([p, q], lr=1e-4, momentum=0.5)
+    for _ in range(100):
+        p.grad, q.grad = torch.ones_like(p), torch.ones_like(q)  # two separate gradients: no flat arena
+        opt.step()
+    st = opt.state[p]
+    assert st["master"].dtype == torch.float32 and st["momentum_buffer"].dtype == torch.float32
+    assert torch.equal(p.data, st["master"].to(torch.bfloat16))
+    assert float(st["master"][0]) < 1 - 0.019 and float(p.data[0]) < 1.0  # 100 steps of about 2e-4 (half an ulp below 1 is 2^-9)
+    assert {k for k, _, _ in launches} == {"sgd_mp"}
 
 
 def test_vgg_fused_feature_path_on_cpu_through_the_native_extension(tmp_path, monkeypatch):
