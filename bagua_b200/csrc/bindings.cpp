@@ -249,6 +249,29 @@ PYBIND11_MODULE(_C, m) {
         .def("set_grad_scale", &AllReduceAdamOp::set_grad_scale)
         .def("steps", &AllReduceAdamOp::steps)
         .def("set_steps", &AllReduceAdamOp::set_steps);
+    py::class_<ShardGradOp, CommOp, std::shared_ptr<ShardGradOp>>(m, "ShardGradOp")
+        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool, LaunchCfg>(), py::arg("comm"),
+             py::arg("grads"), py::arg("g_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("partials_ptr"), py::arg("scale"),
+             py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg"));
+    py::class_<GradNormOp, CommOp, std::shared_ptr<GradNormOp>>(m, "GradNormOp")
+        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, uint64_t, int, uint64_t, uint64_t>(), py::arg("comm"), py::arg("box"), py::arg("box_off"),
+             py::arg("partials_ptr"), py::arg("nslots"), py::arg("extra_ptr"), py::arg("out_ptr"))
+        .def("set_max_norm", &GradNormOp::set_max_norm)
+        .def("calls", &GradNormOp::calls);
+    py::class_<ShardSgdOp, CommOp, std::shared_ptr<ShardSgdOp>>(m, "ShardSgdOp")
+        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(), py::arg("comm"),
+             py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"), py::arg("master_ptr"),
+             py::arg("momentum_ptr"), py::arg("use_multimem"), py::arg("cfg"))
+        .def("set_hyper", &ShardSgdOp::set_hyper)
+        .def("steps", &ShardSgdOp::steps)
+        .def("set_steps", &ShardSgdOp::set_steps);
+    py::class_<ShardAdamOp, CommOp, std::shared_ptr<ShardAdamOp>>(m, "ShardAdamOp")
+        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(),
+             py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
+             py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("use_multimem"), py::arg("cfg"))
+        .def("set_hyper", &ShardAdamOp::set_hyper)
+        .def("steps", &ShardAdamOp::steps)
+        .def("set_steps", &ShardAdamOp::set_steps);
     py::class_<PeerAverageOp, CommOp, std::shared_ptr<PeerAverageOp>>(m, "PeerAverageOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, uint64_t, size_t, int, LaunchCfg>(), py::arg("comm"), py::arg("weights"),
              py::arg("off"), py::arg("out_ptr"), py::arg("bytes"), py::arg("dtype"), py::arg("cfg"))

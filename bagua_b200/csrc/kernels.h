@@ -51,6 +51,19 @@ void launch_all_gather(const PeerCtx& ctx, const PeerBuf& buf, size_t off, size_
 void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
                            float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, float scale, bool zero_grads, bool use_multimem,
                            int nblocks, int nthreads, cudaStream_t stream);
+// Global-norm clipping of the in-bucket optimizers (see shard_grad_kernel): phase A reduce-scatters a bucket into the fp32 gradient
+// `shard` of the owned slice (scaled) and leaves one fp64 Σx² per CTA in partials[block]; grad_norm sums partials[0..nslots) and
+// *extra (nullable), exchanges the per-rank sums through the symmetric `box` (2·kMaxPeers doubles at box_off) and writes
+// out = {total, coef}; phase B applies SGD / Adam to the shard scaled by *coef and all-gathers the weights.
+void launch_shard_grad(const PeerCtx& ctx, const PeerBuf& grads, size_t g_off, size_t bytes, int dtype, float* shard, double* partials, float scale,
+                       bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream);
+void launch_grad_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots, const double* extra, float max_norm,
+                      uint32_t parity, float* out, cudaStream_t stream);
+void launch_shard_sgd(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                      float* master, float* momentum, const SgdParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream);
+void launch_shard_adam(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                       float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, bool use_multimem, int nblocks, int nthreads,
+                       cudaStream_t stream);
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,
                          int nblocks, int nthreads, cudaStream_t stream);
 void launch_peer_barrier(const PeerCtx& ctx, cudaStream_t stream);

@@ -166,6 +166,48 @@ void AllReduceAdamOp::run(Bucket&, StreamHandle stream, int) {
     steps_++;
 }
 
+void ShardGradOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("shard_grad");
+    launch_shard_grad(comm_->ctx(), grads_.buf, g_off_, bytes_, dtype_, reinterpret_cast<float*>(shard_), reinterpret_cast<double*>(partials_), scale_,
+                      zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
+}
+
+void GradNormOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("grad_norm");
+    launch_grad_norm(comm_->ctx(), box_.buf, box_off_, reinterpret_cast<const double*>(partials_), nslots_, reinterpret_cast<const double*>(extra_),
+                     max_norm_, static_cast<uint32_t>(calls_ & 1u), reinterpret_cast<float*>(out_), S(stream));
+    calls_++;
+}
+
+void ShardSgdOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("shard_sgd");
+    SgdParams hp;
+    {
+        std::lock_guard<std::mutex> lk(mu_);
+        hp = hp_;
+    }
+    hp.first_step = steps_ == 0 ? 1 : 0;
+    launch_shard_sgd(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), reinterpret_cast<const float*>(coef_),
+                     reinterpret_cast<float*>(master_), reinterpret_cast<float*>(momentum_), hp, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
+    steps_++;
+}
+
+void ShardAdamOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("shard_adam");
+    AdamParams hp{};
+    {
+        std::lock_guard<std::mutex> lk(mu_);
+        hp.lr = lr_, hp.beta1 = b1_, hp.beta2 = b2_, hp.eps = eps_, hp.weight_decay = wd_, hp.adamw = adamw_ ? 1 : 0;
+    }
+    const double t = static_cast<double>(steps_ + 1);
+    hp.bias_correction1 = static_cast<float>(1.0 - std::pow(static_cast<double>(hp.beta1), t));
+    hp.bias_correction2 = static_cast<float>(1.0 - std::pow(static_cast<double>(hp.beta2), t));
+    launch_shard_adam(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), reinterpret_cast<const float*>(coef_),
+                      reinterpret_cast<float*>(master_), reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), hp, use_mc_, cfg_.nblocks, cfg_.nthreads,
+                      S(stream));
+    steps_++;
+}
+
 int PeerAverageOp::shift_one_peer(int rank, int nranks, int64_t step) {
     const int64_t r = rank, n = nranks;
     if (rank < nranks / 2) return static_cast<int>(((step + r) % ((n + 1) / 2)) + (n / 2));

@@ -221,6 +221,112 @@ private:
     std::mutex mu_;
 };
 
+// Global-norm clipping of the in-bucket optimizers (see shard_grad_kernel). Phase A, in the bucket program: reduce-scatter of the
+// gradients into the fp32 shard of the owned slice, per-CTA fp64 Σx² into `partials` (kMaxCommBlocks doubles), bucket cleared.
+class ShardGradOp final : public CommOp {
+public:
+    ShardGradOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, size_t g_off, size_t bytes, int dtype, uint64_t shard, uint64_t partials, float scale,
+                bool zero_grads, bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), grads_(grads), g_off_(g_off), bytes_(bytes), dtype_(dtype), shard_(shard), partials_(partials), scale_(scale),
+          zero_grads_(zero_grads), use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return "shard_grad_sumsq"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf grads_;
+    size_t g_off_, bytes_;
+    int dtype_;
+    uint64_t shard_, partials_;
+    float scale_;
+    bool zero_grads_, use_mc_;
+    LaunchCfg cfg_;
+};
+
+// The norm exchange: out = {total, coef} (fp32, device) from the `nslots` partials of this rank plus *extra (fp64, the parameters
+// outside the buckets; 0 = none) and the peers' sums. The box is double-buffered by this op's own call counter.
+class GradNormOp final : public CommOp {
+public:
+    GradNormOp(std::shared_ptr<PeerComm> comm, SymmBuf box, size_t box_off, uint64_t partials, int nslots, uint64_t extra, uint64_t out)
+        : comm_(std::move(comm)), box_(box), box_off_(box_off), partials_(partials), nslots_(nslots), extra_(extra), out_(out) {}
+    const char* kind() const override { return "grad_norm"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return false; }  // the box half alternates with the call counter
+    void set_max_norm(float m) { max_norm_ = m; }
+    uint64_t calls() const { return calls_; }
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf box_;
+    size_t box_off_;
+    uint64_t partials_;
+    int nslots_;
+    uint64_t extra_, out_;
+    float max_norm_ = 1.f;
+    uint64_t calls_ = 0;
+};
+
+// Phase B: SGD on the owned shard with the gradient shard·coef, all-gather of the weights. Carries the step counter like
+// AllReduceSgdOp (checkpoints see the same interface).
+class ShardSgdOp final : public CommOp {
+public:
+    ShardSgdOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
+               uint64_t momentum, bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), master_(master),
+          momentum_(momentum), use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return "shard_sgd"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return steps_ > 0; }
+    void set_hyper(float lr, float momentum, float dampening, float weight_decay, bool nesterov) {
+        std::lock_guard<std::mutex> lk(mu_);
+        hp_.lr = lr, hp_.momentum = momentum, hp_.dampening = dampening, hp_.weight_decay = weight_decay, hp_.nesterov = nesterov;
+    }
+    uint64_t steps() const { return steps_; }
+    void set_steps(uint64_t s) { steps_ = s; }
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf weights_;
+    size_t w_off_, bytes_;
+    int dtype_;
+    uint64_t shard_, coef_, master_, momentum_;
+    bool use_mc_;
+    LaunchCfg cfg_;
+    SgdParams hp_{0.01f, 0.f, 0.f, 0.f, 0, 1};
+    uint64_t steps_ = 0;
+    std::mutex mu_;
+};
+
+class ShardAdamOp final : public CommOp {
+public:
+    ShardAdamOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
+                uint64_t exp_avg, uint64_t exp_avg_sq, bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), master_(master),
+          m1_(exp_avg), m2_(exp_avg_sq), use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return "shard_adam"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return false; }
+    void set_hyper(float lr, float beta1, float beta2, float eps, float weight_decay, bool adamw) {
+        std::lock_guard<std::mutex> lk(mu_);
+        lr_ = lr, b1_ = beta1, b2_ = beta2, eps_ = eps, wd_ = weight_decay, adamw_ = adamw;
+    }
+    uint64_t steps() const { return steps_; }
+    void set_steps(uint64_t s) { steps_ = s; }
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf weights_;
+    size_t w_off_, bytes_;
+    int dtype_;
+    uint64_t shard_, coef_, master_, m1_, m2_;
+    bool use_mc_;
+    LaunchCfg cfg_;
+    float lr_ = 1e-3f, b1_ = 0.9f, b2_ = 0.999f, eps_ = 1e-8f, wd_ = 0.f;
+    bool adamw_ = false;
+    uint64_t steps_ = 0;
+    std::mutex mu_;
+};
+
 // Decentralized SGD, shift_one pairing (peer formula: comm_ops/decentralized_full_precision_synchronous.rs:81-85).
 class PeerAverageOp final : public CommOp {
 public:

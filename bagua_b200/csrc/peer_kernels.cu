@@ -233,6 +233,72 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_kernel(PeerCtx ctx, Pee
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// The optimizer update of one 16-byte vector of the owned shard (N lanes at index j·N of the fp32 state), shared by the in-bucket
+// kernels below and by the clipped two-phase kernels further down: g[k]·scale is the gradient the update sees. w receives the new
+// fp32 weights, which the caller publishes.
+// ---------------------------------------------------------------------------------------------------------
+template <int N>
+__device__ __forceinline__ void sgd_update(float* master, float* momentum_buf, size_t j, const float* g, float scale, const SgdParams& hp, float* w) {
+    float m[N];
+    float4* mp = reinterpret_cast<float4*>(master + j * N);
+    float4* mo = reinterpret_cast<float4*>(momentum_buf + j * N);
+#pragma unroll
+    for (int q = 0; q < N / 4; ++q) {
+        float4 a = mp[q];
+        w[4 * q] = a.x, w[4 * q + 1] = a.y, w[4 * q + 2] = a.z, w[4 * q + 3] = a.w;
+        if (hp.momentum != 0.f) {
+            float4 bb = mo[q];
+            m[4 * q] = bb.x, m[4 * q + 1] = bb.y, m[4 * q + 2] = bb.z, m[4 * q + 3] = bb.w;
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+        float d = g[k] * scale + hp.weight_decay * w[k];
+        if (hp.momentum != 0.f) {
+            m[k] = hp.first_step ? d : hp.momentum * m[k] + (1.f - hp.dampening) * d;
+            d = hp.nesterov ? d + hp.momentum * m[k] : m[k];
+        }
+        w[k] -= hp.lr * d;
+    }
+#pragma unroll
+    for (int q = 0; q < N / 4; ++q) {
+        mp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+        if (hp.momentum != 0.f) mo[q] = make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]);
+    }
+}
+
+// Adam / AdamW, update rule identical to flat_adam_kernel (multi_tensor.cu) / torch.optim.Adam[W]; inv_bc1 = 1/(1−β1^t),
+// inv_sqrt_bc2 = 1/sqrt(1−β2^t).
+template <int N>
+__device__ __forceinline__ void adam_update(float* master, float* exp_avg, float* exp_avg_sq, size_t j, const float* g, float scale, const AdamParams& hp,
+                                            float inv_bc1, float inv_sqrt_bc2, float* w) {
+    float4* wp = reinterpret_cast<float4*>(master + j * N);
+    float4* ap = reinterpret_cast<float4*>(exp_avg + j * N);
+    float4* bp = reinterpret_cast<float4*>(exp_avg_sq + j * N);
+#pragma unroll
+    for (int q = 0; q < N / 4; ++q) {
+        float4 ww = wp[q], aa = ap[q], bb = bp[q];
+        float wv[4] = {ww.x, ww.y, ww.z, ww.w}, av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            float gg = g[4 * q + k] * scale;
+            if (hp.adamw)
+                wv[k] *= (1.f - hp.lr * hp.weight_decay);
+            else
+                gg += hp.weight_decay * wv[k];
+            av[k] = hp.beta1 * av[k] + (1.f - hp.beta1) * gg;
+            bv[k] = hp.beta2 * bv[k] + (1.f - hp.beta2) * gg * gg;
+            const float denom = sqrtf(bv[k]) * inv_sqrt_bc2 + hp.eps;
+            wv[k] -= (hp.lr * inv_bc1) * (av[k] / denom);
+            w[4 * q + k] = wv[k];
+        }
+        wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
+        ap[q] = make_float4(av[0], av[1], av[2], av[3]);
+        bp[q] = make_float4(bv[0], bv[1], bv[2], bv[3]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // Gradient reduce-scatter  →  SGD(momentum) on the owned 1/P slice  →  all-gather of the updated WEIGHTS,
 // in one kernel. Each rank keeps fp32 master weights and momentum only for its own slice (optimizer state is
 // sharded P ways), the gradient bucket is zeroed for the next iteration on the way out, and the optimizer step
@@ -248,33 +314,8 @@ __global__ void __launch_bounds__(512)
     const Slicing sl(total_vecs, P);
     if (ok) {
         reduce_owned_slice<T, P, USE_MC, kOptimizerUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t v, size_t j, float* g) {
-            // optimizer state of the owned slice: index j*N within the shard
-            float w[N], m[N];
-            float4* mp = reinterpret_cast<float4*>(master + j * N);
-            float4* mo = reinterpret_cast<float4*>(momentum_buf + j * N);
-#pragma unroll
-            for (int q = 0; q < N / 4; ++q) {
-                float4 a = mp[q];
-                w[4 * q] = a.x, w[4 * q + 1] = a.y, w[4 * q + 2] = a.z, w[4 * q + 3] = a.w;
-                if (hp.momentum != 0.f) {
-                    float4 bb = mo[q];
-                    m[4 * q] = bb.x, m[4 * q + 1] = bb.y, m[4 * q + 2] = bb.z, m[4 * q + 3] = bb.w;
-                }
-            }
-#pragma unroll
-            for (int k = 0; k < N; ++k) {
-                float d = g[k] * scale + hp.weight_decay * w[k];
-                if (hp.momentum != 0.f) {
-                    m[k] = hp.first_step ? d : hp.momentum * m[k] + (1.f - hp.dampening) * d;
-                    d = hp.nesterov ? d + hp.momentum * m[k] : m[k];
-                }
-                w[k] -= hp.lr * d;
-            }
-#pragma unroll
-            for (int q = 0; q < N / 4; ++q) {
-                mp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-                if (hp.momentum != 0.f) mo[q] = make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]);
-            }
+            float w[N];
+            sgd_update<N>(master, momentum_buf, j, g, scale, hp, w);
             publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
         });
         ok = peer_barrier(ctx, e0 + 2);
@@ -302,31 +343,8 @@ __global__ void __launch_bounds__(512)
     if (ok) {
         const float inv_bc1 = 1.f / hp.bias_correction1, inv_sqrt_bc2 = rsqrtf(hp.bias_correction2);
         reduce_owned_slice<T, P, USE_MC, kOptimizerUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t v, size_t j, float* g) {
-            float4* wp = reinterpret_cast<float4*>(master + j * N);
-            float4* ap = reinterpret_cast<float4*>(exp_avg + j * N);
-            float4* bp = reinterpret_cast<float4*>(exp_avg_sq + j * N);
             float w[N];
-#pragma unroll
-            for (int q = 0; q < N / 4; ++q) {
-                float4 ww = wp[q], aa = ap[q], bb = bp[q];
-                float wv[4] = {ww.x, ww.y, ww.z, ww.w}, av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    float gg = g[4 * q + k] * scale;
-                    if (hp.adamw)
-                        wv[k] *= (1.f - hp.lr * hp.weight_decay);
-                    else
-                        gg += hp.weight_decay * wv[k];
-                    av[k] = hp.beta1 * av[k] + (1.f - hp.beta1) * gg;
-                    bv[k] = hp.beta2 * bv[k] + (1.f - hp.beta2) * gg * gg;
-                    const float denom = sqrtf(bv[k]) * inv_sqrt_bc2 + hp.eps;
-                    wv[k] -= (hp.lr * inv_bc1) * (av[k] / denom);
-                    w[4 * q + k] = wv[k];
-                }
-                wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
-                ap[q] = make_float4(av[0], av[1], av[2], av[3]);
-                bp[q] = make_float4(bv[0], bv[1], bv[2], bv[3]);
-            }
+            adam_update<N>(master, exp_avg, exp_avg_sq, j, g, scale, hp, inv_bc1, inv_sqrt_bc2, w);
             publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
         });
         ok = peer_barrier(ctx, e0 + 2);
@@ -336,6 +354,152 @@ __global__ void __launch_bounds__(512)
         for_each_striped<P>(sl, [&](size_t v) { st_stream16(mine + v * 16, make_uint4(0, 0, 0, 0)); });
     }
     store_epoch(ctx, e0 + 2);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Global-norm gradient clipping for the in-bucket optimizers. No shard may be updated before the norm over every bucket of every
+// rank is known, so the single in-bucket kernel above becomes two phases around a norm exchange:
+//   A  shard_grad_kernel, per bucket, inside backward on the comm stream: the owned-slice reduction (same order and the same
+//      multimem / peer ld choice as allreduce_{sgd,adam}_kernel) scaled by `scale` → the fp32 gradient of the owned slice in
+//      `shard`; one fp64 Σx² per CTA in partials[block] (no atomics: reproducible, nothing to reset between steps); the bucket is
+//      cleared after the closing barrier.
+//   N  grad_norm_kernel, once per step: the rank's Σ over all partials (+ the parameters outside the buckets) → slot [rank] of
+//      every peer's norm box → barrier → Σ over slots 0 .. P-1 in rank order, so every rank computes the same bits → total, coef.
+//   B  shard_{sgd,adam}_kernel, per bucket: the update of the shard scaled by coef (read from device memory: the host never sees
+//      the norm) → all-gather of the weights → closing barrier, so no rank's trainer reads weights a peer is still writing.
+// ---------------------------------------------------------------------------------------------------------
+template <typename T, int P, bool USE_MC>
+__global__ void __launch_bounds__(512)
+    shard_grad_kernel(PeerCtx ctx, PeerBuf grads, size_t g_off, size_t total_vecs, float* shard, double* partials, float scale, int zero_grads) {
+    __shared__ double s_warp[512 / 32];
+    const uint32_t e0 = load_epoch(ctx);
+    bool ok = peer_barrier(ctx, e0 + 1);
+    constexpr int N = Vec16<T>::N;
+    const Slicing sl(total_vecs, P);
+    double ss = 0.0;
+    if (ok) {
+        reduce_owned_slice<T, P, USE_MC, kReduceUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t, size_t j, float* g) {
+            float4* sp = reinterpret_cast<float4*>(shard + j * N);
+#pragma unroll
+            for (int k = 0; k < N; ++k) {
+                g[k] *= scale;
+                ss += static_cast<double>(g[k]) * static_cast<double>(g[k]);
+            }
+#pragma unroll
+            for (int q = 0; q < N / 4; ++q) sp[q] = make_float4(g[4 * q], g[4 * q + 1], g[4 * q + 2], g[4 * q + 3]);
+        });
+        ok = peer_barrier(ctx, e0 + 2);
+    }
+    // the CTA's Σx² in a fixed order: a shuffle tree per warp, then the warps in index order
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = ss;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (unsigned w = 0; w < blockDim.x / 32; ++w) t += s_warp[w];
+        partials[blockIdx.x] = t;
+    }
+    if (ok && zero_grads) {
+        char* mine = grads.ptr[ctx.rank] + g_off;
+        for_each_striped<P>(sl, [&](size_t v) { st_stream16(mine + v * 16, make_uint4(0, 0, 0, 0)); });
+    }
+    store_epoch(ctx, e0 + 2);
+}
+
+__device__ __forceinline__ void st_peer_f64(void* p, double v) {
+    asm volatile("st.relaxed.sys.global.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
+}
+__device__ __forceinline__ double ld_peer_f64(const void* p) {
+    double v;
+    asm volatile("ld.relaxed.sys.global.f64 %0, [%1];" : "=d"(v) : "l"(p) : "memory");
+    return v;
+}
+
+// One CTA of kNormThreads threads. The box holds [2][kMaxPeers] doubles per rank, double-buffered by the host's call counter
+// (`parity`) like the one-shot staging area: a rank can only write a half again two calls later, after every peer has left the
+// call in between, so no closing barrier is needed. out = {total, coef}, coef = min(max_norm / (total + 1e-6), 1) in fp32 with
+// torch's operation order (reciprocal, then the product); a NaN norm gives a NaN coef, as in torch.
+constexpr int kNormThreads = 256;
+__global__ void __launch_bounds__(kNormThreads) grad_norm_kernel(PeerCtx ctx, PeerBuf box, size_t box_off, const double* partials, int nslots,
+                                                                 const double* extra, float max_norm, uint32_t parity, float* out) {
+    __shared__ double s_sum[kNormThreads];
+    const uint32_t e0 = load_epoch(ctx);
+    double s = 0.0;
+    for (int i = threadIdx.x; i < nslots; i += kNormThreads) s += partials[i];
+    s_sum[threadIdx.x] = s;
+    __syncthreads();
+#pragma unroll
+    for (int o = kNormThreads / 2; o > 0; o >>= 1) {
+        if (threadIdx.x < o) s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
+        __syncthreads();
+    }
+    const size_t half = box_off + static_cast<size_t>(parity & 1u) * kMaxPeers * sizeof(double);
+    if (threadIdx.x < ctx.world) {
+        const double mine = s_sum[0] + (extra != nullptr ? *extra : 0.0);
+        st_peer_f64(box.ptr[threadIdx.x] + half + ctx.rank * sizeof(double), mine);
+    }
+    const bool ok = peer_barrier(ctx, e0 + 1);
+    if (threadIdx.x == 0) {
+        float total = __int_as_float(0x7fc00000), coef = total;
+        if (ok) {
+            const char* mybox = box.ptr[ctx.rank] + half;
+            double sum = 0.0;
+            for (int p = 0; p < ctx.world; ++p) sum += ld_peer_f64(mybox + p * sizeof(double));
+            total = static_cast<float>(sqrt(sum));
+            const float c = __fmul_rn(__frcp_rn(__fadd_rn(total, 1e-6f)), max_norm);
+            coef = c > 1.f ? 1.f : c;
+        }
+        out[0] = total;
+        out[1] = coef;
+    }
+    store_epoch(ctx, e0 + 1);
+}
+
+// Phase B: the shard's own vectors, U-unrolled like the reduction walk (all shard loads of an iteration before any update).
+template <typename T, int P, bool USE_MC, typename Update>
+__device__ __forceinline__ void update_owned_shard(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, const Slicing& sl, const float* shard,
+                                                   Update&& update) {
+    constexpr int N = Vec16<T>::N;
+    using Raw = float4[N / 4];
+    walk_owned_slice<kOptimizerUnroll<P, USE_MC>, Raw>(
+        sl, ctx.rank,
+        [&](Raw& raw, size_t v) {
+            const float4* sp = reinterpret_cast<const float4*>(shard + (v - static_cast<size_t>(ctx.rank) * sl.vpr) * N);
+#pragma unroll
+            for (int q = 0; q < N / 4; ++q) raw[q] = sp[q];
+        },
+        [&](Raw& raw, size_t v, size_t j) {
+            float g[N], w[N];
+#pragma unroll
+            for (int q = 0; q < N / 4; ++q) g[4 * q] = raw[q].x, g[4 * q + 1] = raw[q].y, g[4 * q + 2] = raw[q].z, g[4 * q + 3] = raw[q].w;
+            update(j, g, w);
+            publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
+        });
+}
+
+template <typename T, int P, bool USE_MC>
+__global__ void __launch_bounds__(512) shard_sgd_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
+                                                        const float* coef, float* master, float* momentum_buf, SgdParams hp) {
+    const uint32_t e0 = load_epoch(ctx);
+    const float c = *coef;
+    update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard,
+                                     [&](size_t j, const float* g, float* w) { sgd_update<Vec16<T>::N>(master, momentum_buf, j, g, c, hp, w); });
+    peer_barrier(ctx, e0 + 1);
+    store_epoch(ctx, e0 + 1);
+}
+
+template <typename T, int P, bool USE_MC>
+__global__ void __launch_bounds__(512) shard_adam_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
+                                                         const float* coef, float* master, float* exp_avg, float* exp_avg_sq, AdamParams hp) {
+    const uint32_t e0 = load_epoch(ctx);
+    const float c = *coef;
+    const float inv_bc1 = 1.f / hp.bias_correction1, inv_sqrt_bc2 = rsqrtf(hp.bias_correction2);
+    update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard, [&](size_t j, const float* g, float* w) {
+        adam_update<Vec16<T>::N>(master, exp_avg, exp_avg_sq, j, g, c, hp, inv_bc1, inv_sqrt_bc2, w);
+    });
+    peer_barrier(ctx, e0 + 1);
+    store_epoch(ctx, e0 + 1);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -634,6 +798,61 @@ void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerB
         });
     });
     check_launch("allreduce_adam");
+}
+
+void launch_shard_grad(const PeerCtx& ctx, const PeerBuf& grads, size_t g_off, size_t bytes, int dtype, float* shard, double* partials, float scale,
+                       bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream) {
+    const size_t vecs = peer_vecs("shard_grad", bytes, g_off, 0, nblocks);
+    if (nthreads % 32 || nthreads > 512) throw std::runtime_error("bagua: shard_grad needs whole warps, at most 512 threads");
+    if (vecs == 0) return;
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(ctx.world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                shard_grad_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
+                    ctx, grads, g_off, vecs, shard, partials, scale, zero_grads ? 1 : 0);
+            });
+        });
+    });
+    check_launch("shard_grad");
+}
+
+void launch_grad_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots, const double* extra, float max_norm,
+                      uint32_t parity, float* out, cudaStream_t stream) {
+    if (box_off % 8) throw std::runtime_error("bagua: grad_norm box offset must be 8-byte aligned");
+    grad_norm_kernel<<<1, kNormThreads, 0, stream>>>(ctx, box, box_off, partials, nslots, extra, max_norm, parity, out);
+    check_launch("grad_norm");
+}
+
+void launch_shard_sgd(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                      float* master, float* momentum, const SgdParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream) {
+    const size_t vecs = peer_vecs("shard_sgd", bytes, w_off, 0, nblocks);
+    if (vecs == 0) return;
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(ctx.world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                shard_sgd_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
+                    ctx, weights, w_off, vecs, shard, coef, master, momentum, hp);
+            });
+        });
+    });
+    check_launch("shard_sgd");
+}
+
+void launch_shard_adam(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                       float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, bool use_multimem, int nblocks, int nthreads,
+                       cudaStream_t stream) {
+    const size_t vecs = peer_vecs("shard_adam", bytes, w_off, 0, nblocks);
+    if (hp.amsgrad) throw std::runtime_error("bagua: shard_adam does not implement amsgrad");
+    if (vecs == 0) return;
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(ctx.world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                shard_adam_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
+                    ctx, weights, w_off, vecs, shard, coef, master, exp_avg, exp_avg_sq, hp);
+            });
+        });
+    });
+    check_launch("shard_adam");
 }
 
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,

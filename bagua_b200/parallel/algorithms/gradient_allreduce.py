@@ -91,6 +91,7 @@ class _ShardedStateMixin:
     a checkpoint does not depend on the world size or on the bucket boundaries (autotune may move them)."""
 
     _kind = "sgd"
+    max_grad_norm = None
 
     @property
     def collective_state_dict(self) -> bool:
@@ -150,19 +151,108 @@ class _ShardedStateMixin:
             if hi > lo:
                 rec["state"][0][: hi - lo].copy_(rec["weights"][lo:hi].float())
 
-    def _step_uncovered(self):
-        """Parameters that no bucket kernel updates — MoE experts (excluded from data parallelism), ignored parameters —
-        get the ordinary fused update here; their gradients are cleared like the bucketed ones."""
+    def _uncovered(self):
         candidates = getattr(self, "_uncovered_cache", None)
         if candidates is None:  # the parameter list is static between (re-)initialisations: looked up once, usually empty
             covered = getattr(self, "_covered", set())
             candidates = self._uncovered_cache = [p for g in self.param_groups for p in g["params"] if id(p) not in covered]
-        left = [p for p in candidates if p.grad is not None]
+        return [p for p in candidates if p.grad is not None]
+
+    def _step_uncovered(self, coef=None):
+        """Parameters that no bucket kernel updates — MoE experts (excluded from data parallelism), ignored parameters —
+        get the ordinary fused update here (their gradients scaled by the clipping coefficient ``coef`` first, when given);
+        their gradients are cleared like the bucketed ones."""
+        left = self._uncovered()
         if left:
-            super().step(only={id(p) for p in left})
             import torch
 
+            if coef is not None:
+                torch._foreach_mul_([p.grad for p in left], coef)
+            super().step(only={id(p) for p in left})
             torch._foreach_zero_([p.grad for p in left])
+
+    # ---- global gradient-norm clipping (``max_grad_norm``) ---------------------------------------------------------------
+    @property
+    def last_grad_norm(self):
+        """Global L2 norm of the averaged gradient at the last step that clipped: a device fp32 0-d tensor with the same bits on
+        every rank, overwritten by the next step (no host synchronisation). ``None`` before the first one."""
+        return getattr(self, "_last_norm", None)
+
+    def clip_grad_norm_(self, max_norm: float, norm_type: float = 2.0):
+        """Clip by the global L2 norm of the averaged gradient with bound ``max_norm`` for this step and return the norm (device
+        fp32 0-d tensor), like ``torch.nn.utils.clip_grad_norm_`` after a data-parallel all-reduce.
+
+        With the bucket kernels live the gradients are consumed during backward, so this needs an optimizer built with
+        ``max_grad_norm``: the call then computes the norm that the following ``step()`` applies (``step()`` computes it itself
+        when this is not called). Without a peer engine the gradients are ordinary all-reduced tensors and the flat path clips
+        them in place."""
+        live = bool(getattr(self, "_comm_ops", None))
+        if float(norm_type) != 2.0 and (live or self.max_grad_norm is not None):
+            raise ValueError(f"the sharded fused optimizers clip by the L2 norm only, got norm_type={norm_type}")
+        if not live:
+            total = super().clip_grad_norm_(max_norm, norm_type)
+            self._norm_pending, self._last_norm = True, total
+            return total
+        if getattr(self, "_clip", None) is None:
+            raise RuntimeError("the in-bucket optimizer applied this step's update during backward, so its gradients cannot be clipped "
+                               "afterwards; construct it with max_grad_norm=... (make_sharded_fused_sgd / make_sharded_fused_adam) to clip "
+                               "on this path")
+        return self._launch_norm(max_norm).clone()
+
+    def _launch_norm(self, max_norm):
+        import torch
+
+        from ...core import native
+
+        clip = self._clip
+        loose = [p.grad for p in self._uncovered()]
+        if loose:   # each rank adds the local Σx² of its parameters outside the buckets: every expert counts once in the total
+            clip["extra"].copy_(torch.stack([torch.linalg.vector_norm(g, dtype=torch.float64) for g in loose]).square().sum())
+            clip["extra_set"] = True
+        elif clip["extra_set"]:
+            clip["extra"].zero_()
+            clip["extra_set"] = False
+        clip["norm_op"].set_max_norm(float(max_norm))
+        dev = clip["out"].device
+        native().run_op(clip["norm_op"], torch.cuda.current_stream(dev).cuda_stream, dev.index)
+        self.kernel_launches += 1
+        self._norm_pending = True
+        self._last_norm = clip["out"][0]
+        return self._last_norm
+
+    def step(self, closure=None):
+        """Without clipping the update already ran in the bucket kernels of this iteration's backward: publish the
+        hyper-parameters for the next one and step the parameters outside the buckets. With ``max_grad_norm``: the norm
+        exchange (unless ``clip_grad_norm_`` ran it), then the clipped update of every bucket's shard and the all-gather of the
+        weights, then the parameters outside the buckets, all on the current stream."""
+        if not self._comm_ops:
+            if self.max_grad_norm is not None and not getattr(self, "_norm_pending", False):
+                self._last_norm = super().clip_grad_norm_(self.max_grad_norm)
+            self._norm_pending = False
+            return super().step(closure)
+        self._sync_hyper()
+        coef = None
+        if getattr(self, "_clip", None) is not None:
+            # Ordering: the post-backward hook made this stream wait for the comm stream, so every phase-A bucket kernel (shard +
+            # partials) has finished; the next iteration's bucket launches wait for ready events recorded after this step() on
+            # this stream. So phase A, the norm exchange and phase B of one PeerComm stay totally ordered, the shards and the
+            # partials are never overwritten while read, and the weights are all-gathered before the next forward reads them.
+            import torch
+
+            from ...core import native
+
+            if not getattr(self, "_norm_pending", False):
+                self._launch_norm(self.max_grad_norm)
+            self._norm_pending = False
+            dev = self._clip["out"].device
+            C, stream = native(), torch.cuda.current_stream(dev).cuda_stream
+            for op in self._comm_ops:
+                C.run_op(op, stream, dev.index)
+            coef = self._clip["out"][1]
+        self._step_uncovered(coef)
+        self._grads_zeroed = True
+        self.kernel_launches += len(self._comm_ops)
+        return None
 
     def _register_shard(self, rec):
         if not hasattr(self, "_shards"):
@@ -185,12 +275,23 @@ class ShardedFusedSGD(object):
     """Marker mix-in: see :func:`make_sharded_fused_sgd`."""
 
 
-def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False):
+def _check_bound(max_grad_norm):
+    if max_grad_norm is not None and not float(max_grad_norm) > 0:
+        raise ValueError(f"max_grad_norm must be a positive number or None, got {max_grad_norm}")
+    return None if max_grad_norm is None else float(max_grad_norm)
+
+
+def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, max_grad_norm=None):
     """SGD whose update runs *inside* each bucket's NVSwitch kernel (``allreduce_sgd_kernel``): reduce-scatter of the
     gradients → SGD(momentum) on this rank's 1/N shard with fp32 master weights → all-gather of the updated weights, one
     launch per bucket, overlapped with the rest of backward.  Optimizer state is sharded N ways (ZeRO-1-like) and the
     gradient bucket is cleared on the way out.  Use together with ``FusedGradientAllReduceAlgorithm``; with one process (or
-    without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedSGD`."""
+    without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedSGD`.
+
+    ``max_grad_norm``: clip by the global L2 norm of the averaged gradient, as ``torch.nn.utils.clip_grad_norm_`` after a
+    data-parallel all-reduce.  The bucket kernels then only reduce-scatter the gradients into an fp32 shard during backward
+    (4 bytes per element / N of extra memory) and ``step()`` runs the norm exchange and the clipped update; see
+    ``docs/algorithms.md``."""
     from ...ops.optim import FusedSGD
 
     class _ShardedFusedSGD(_ShardedStateMixin, FusedSGD, ShardedFusedSGD):
@@ -198,7 +299,7 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
 
         def __init__(self, *a, **k):
             super().__init__(*a, **k)
-            self._comm_ops = []   # AllReduceSgdOp per bucket once the algorithm has taken over
+            self._comm_ops = []   # the update op of every bucket (AllReduceSgdOp, or ShardSgdOp when clipping) once the algorithm has taken over
             self._shards = []
 
         def _sync_hyper(self):
@@ -207,28 +308,21 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
                 g = self.param_groups[groups[i] if i < len(groups) else 0]   # every bucket op serves one parameter group
                 op.set_hyper(float(g["lr"]), float(g["momentum"]), float(g["dampening"]), float(g["weight_decay"]), bool(g["nesterov"]))
 
-        def step(self, closure=None):
-            if not self._comm_ops:
-                return super().step(closure)
-            # the update already happened in the bucket kernels of this iteration; publish hyper-parameters for the next
-            self._sync_hyper()
-            self._step_uncovered()
-            self._grads_zeroed = True
-            self.kernel_launches += len(self._comm_ops)
-            return None
-
-    return _ShardedFusedSGD(params, lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
-                            master_weights=True, zero_grad_in_step=True)
+    opt = _ShardedFusedSGD(params, lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
+                           master_weights=True, zero_grad_in_step=True)
+    opt.max_grad_norm = _check_bound(max_grad_norm)
+    return opt
 
 
 class ShardedFusedAdam(object):
     """Marker mix-in: see :func:`make_sharded_fused_adam`."""
 
 
-def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False):
+def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False, max_grad_norm=None):
     """Adam / AdamW counterpart of :func:`make_sharded_fused_sgd`: the update of this rank's 1/N shard (fp32 master weights
     and both moments) runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_adam_kernel``).  With one
-    process (or without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedAdam`."""
+    process (or without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedAdam`.  ``max_grad_norm``: see
+    :func:`make_sharded_fused_sgd`."""
     from ...ops.optim import FusedAdam
 
     class _ShardedFusedAdam(_ShardedStateMixin, FusedAdam, ShardedFusedAdam):
@@ -245,17 +339,10 @@ def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weigh
                 g = self.param_groups[groups[i] if i < len(groups) else 0]
                 op.set_hyper(float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]), bool(g["adamw"]))
 
-        def step(self, closure=None):
-            if not self._comm_ops:
-                return super().step(closure)
-            self._sync_hyper()
-            self._step_uncovered()
-            self._grads_zeroed = True
-            self.kernel_launches += len(self._comm_ops)
-            return None
-
-    return _ShardedFusedAdam(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, adamw=adamw, master_weights=True,
-                             zero_grad_in_step=True)
+    opt = _ShardedFusedAdam(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, adamw=adamw, master_weights=True,
+                            zero_grad_in_step=True)
+    opt.max_grad_norm = _check_bound(max_grad_norm)
+    return opt
 
 
 class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
@@ -296,6 +383,7 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         opt._shards = []
         opt._covered = set()
         opt._uncovered_cache = None
+        opt._clip = None
 
     def tensors_to_buckets(self, tensors, do_flatten):
         from ...bucket import BaguaBucket
@@ -321,6 +409,26 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
                 bk._fused_group = gi
                 buckets.append(bk)
         return buckets
+
+    def _clip_state(self, eng, bagua_ddp, bucket, device):
+        """Buffers of the norm exchange, shared by all buckets: fp64 partial sums [bucket][CTA] (slots of unused CTAs stay 0), the
+        fp64 Σx² of the parameters outside the buckets, out = {total, coef} in fp32, and the symmetric norm box (2·MAX_PEERS doubles,
+        freed with the first bucket's other symmetric slices when the buckets are rebuilt)."""
+        import torch
+
+        from ...core import native
+
+        C = native()
+        st = {"partials": torch.zeros(len(bagua_ddp.bagua_buckets), C.MAX_COMM_BLOCKS, dtype=torch.float64, device=device),
+              "extra": torch.zeros((), dtype=torch.float64, device=device), "extra_set": False,
+              "out": torch.zeros(2, dtype=torch.float32, device=device)}
+        box = eng.alloc(2 * C.MAX_PEERS * 8)
+        bucket._companion_slices.append(box)
+        st["box"] = box
+        st["norm_op"] = C.GradNormOp(eng.comm, box.buf, box.offset, st["partials"].data_ptr(), st["partials"].numel(), st["extra"].data_ptr(),
+                                     st["out"].data_ptr())
+        self.optimizer._clip = st
+        return st
 
     def init_operations(self, bagua_ddp, bucket):
         import os
@@ -378,18 +486,36 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         # shard per rank and wants 64 (VGG16 N=1 self-peer: 8 CTAs 5.43 ms/step, 32: 4.34, 64: 4.23 = the flat-optimizer path)
         cfg = eng.launch_cfg("multimem" if use_mc else "two_shot", nbytes, blocks=int(os.environ.get("BAGUA_FUSED_BLOCKS", "0")) or (16 if use_mc else 64))
         scale = (1.0 / n) if self.average else 1.0
-        if is_adam:
-            second = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
-            bucket._fused_state = (master, momentum, second)
-            op = C.AllReduceAdamOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, dtype_code(flat.dtype),
+        code = dtype_code(flat.dtype)
+        second = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device) if is_adam else None
+        bucket._fused_state = (master, momentum, second) if is_adam else (master, momentum)
+        clip = opt.max_grad_norm is not None
+        if clip:
+            # phase A in the bucket program (reduce-scatter into the fp32 shard + per-CTA Σx²); the update op runs in step()
+            st = opt._clip if getattr(opt, "_clip", None) is not None else self._clip_state(eng, bagua_ddp, bucket, flat.device)
+            shard = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
+            bucket._clip_shard = shard
+            row = st["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
+            red = C.ShardGradOp(eng.comm, bucket._slice.buf, bucket._slice.offset, nbytes, code, shard.data_ptr(), row.data_ptr(), scale, True, use_mc, cfg)
+            bucket.backend_bucket.append_op(red)
+            bucket._ops_keepalive.append(red)
+            coef_ptr = st["out"][1:].data_ptr()
+            if is_adam:
+                op = C.ShardAdamOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
+                                   second.data_ptr(), use_mc, cfg)
+            else:
+                op = C.ShardSgdOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
+                                  use_mc, cfg)
+        elif is_adam:
+            op = C.AllReduceAdamOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                    master.data_ptr(), momentum.data_ptr(), second.data_ptr(), scale, True, use_mc, cfg)
         else:
-            bucket._fused_state = (master, momentum)
-            op = C.AllReduceSgdOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, dtype_code(flat.dtype),
+            op = C.AllReduceSgdOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                   master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
-        bucket.backend_bucket.append_op(op)
+        if not clip:
+            bucket.backend_bucket.append_op(op)
         bucket._ops_keepalive.append(op)
-        bucket.allreduce_variant = ("fused_adam_" if is_adam else "fused_sgd_") + ("multimem" if use_mc else "two_shot")
+        bucket.allreduce_variant = ("fused_adam_" if is_adam else "fused_sgd_") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
         opt._comm_ops.append(op)
         if not hasattr(opt, "_comm_groups"):
             opt._comm_groups = []

@@ -45,7 +45,7 @@ import bagua_b200 as bagua  # noqa: E402
 from bagua_b200 import models  # noqa: E402
 from bagua_b200.contrib import LoadBalancingDistributedSampler  # noqa: E402
 from bagua_b200.parallel.algorithms import Algorithm, q_adam  # noqa: E402
-from bagua_b200.parallel.algorithms.gradient_allreduce import FusedGradientAllReduceAlgorithm, make_sharded_fused_adam  # noqa: E402
+from bagua_b200.parallel.algorithms.gradient_allreduce import FusedGradientAllReduceAlgorithm, ShardedFusedAdam, make_sharded_fused_adam  # noqa: E402
 
 _spec = importlib.util.spec_from_file_location("bagua_example_squad_utils", os.path.join(HERE, "squad_utils.py"))
 su = importlib.util.module_from_spec(_spec)
@@ -251,7 +251,8 @@ def make_optimizer(args, model, cuda, world):
         opt = q_adam.QAdamOptimizer(model.parameters(), lr=args.learning_rate, warmup_steps=100, eps=args.adam_epsilon, weight_decay=args.weight_decay)
         return opt, q_adam.QAdamAlgorithm(opt)
     if args.fused_shard and cuda and args.algorithm == "gradient_allreduce":
-        opt = make_sharded_fused_adam(groups, lr=args.learning_rate, eps=args.adam_epsilon, adamw=True)   # buckets are cut per parameter group
+        opt = make_sharded_fused_adam(groups, lr=args.learning_rate, eps=args.adam_epsilon, adamw=True,   # buckets are cut per parameter group
+                                      max_grad_norm=args.max_grad_norm if args.max_grad_norm > 0 else None)   # clipped inside step()
         return opt, FusedGradientAllReduceAlgorithm(opt)
     if cuda and not args.fuse_optimizer:
         opt = bagua.ops.FusedAdam(groups, lr=args.learning_rate, eps=args.adam_epsilon, adamw=True)
@@ -311,6 +312,8 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
 
         return torch.cuda.nvtx.range(name) if (cuda and args.prof >= 0) else contextlib.nullcontext()
 
+    sharded = isinstance(optimizer, ShardedFusedAdam)
+    grad_norm = None
     step, seen_iters, loss_sum, loss_n, t_log, done = 0, 0, 0.0, 0, time.time(), False
     last_loss = None
     for epoch in range(epochs):
@@ -333,11 +336,13 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
                 if not last_micro:
                     continue
                 with nvtx("optimizer.step()"):
-                    if args.max_grad_norm > 0 and args.algorithm != "qadam" and not args.fused_shard:
+                    if args.max_grad_norm > 0 and args.algorithm != "qadam" and not sharded:
                         if args.algorithm in ("gradient_allreduce", "bytegrad"):
                             model.bagua_ddp.wait_pending_comm_ops()   # clip the COMMUNICATED gradient (the reference clips after backward, :262-267)
-                        torch.nn.utils.clip_grad_norm_(model.parameters(), args.max_grad_norm)
+                        grad_norm = torch.nn.utils.clip_grad_norm_(model.parameters(), args.max_grad_norm)
                     optimizer.fuse_step() if args.fuse_optimizer else optimizer.step()
+                    if sharded:   # the sharded optimizer clipped inside step() (max_grad_norm)
+                        grad_norm = optimizer.last_grad_norm
                     scheduler.step()
                     optimizer.zero_grad()
             step += 1
@@ -345,7 +350,8 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
             if args.logging_steps > 0 and step % args.logging_steps == 0:
                 loss_sum, loss_n = loss_sum + last_loss.item(), loss_n + 1
                 rate = args.per_gpu_train_batch_size * accum * world * args.logging_steps / max(time.time() - t_log, 1e-9)
-                log.info("epoch %d step %d/%d loss %.4f lr %.3g %.1f samples/s", epoch, step, total, last_loss.item(), scheduler.get_last_lr()[0], rate)
+                gn = "-" if grad_norm is None else f"{float(grad_norm):.4f}"
+                log.info("epoch %d step %d/%d loss %.4f lr %.3g grad norm %s %.1f samples/s", epoch, step, total, last_loss.item(), scheduler.get_last_lr()[0], gn, rate)
                 if args.evaluate_during_training:
                     res = evaluate(args, model, tokenizer, dev, rank, world, prefix=str(step))
                     log.info("  step %d: exact %.2f f1 %.2f", step, res["exact"], res["f1"])
