@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstddef>
 #include <cstdint>
 #include <type_traits>
@@ -32,6 +33,26 @@ struct AdamParams {
     int adamw;               // decoupled weight decay
     int amsgrad;             // unsupported (kept for ABI stability)
 };
+
+// LAMB (You et al. 2019) with apex FusedLAMB's defaults: bias correction, decoupled weight decay inside the update direction, the
+// trust ratio ‖w‖/‖u‖ applied only where weight_decay != 0 (see lamb.cuh).
+struct LambParams {
+    float lr;
+    float beta1;
+    float beta2;
+    float eps;
+    float weight_decay;
+    float bias_correction1;  // 1 - beta1^t
+    float bias_correction2;  // 1 - beta2^t
+};
+
+inline LambParams lamb_params(float lr, float beta1, float beta2, float eps, float weight_decay, uint64_t step) {
+    LambParams p{lr, beta1, beta2, eps, weight_decay, 0.f, 0.f};
+    const double t = static_cast<double>(step);  // as the in-bucket Adam ops compute them: in double, rounded once
+    p.bias_correction1 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta1), t));
+    p.bias_correction2 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta2), t));
+    return p;
+}
 
 // ---- peer kernels (peer_kernels.cu) ------------------------------------------------------------------------
 void launch_allreduce(const PeerCtx& ctx, const PeerBuf& src, const PeerBuf& dst, size_t src_off, size_t dst_off, size_t bytes,
@@ -64,6 +85,17 @@ void launch_shard_sgd(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, 
 void launch_shard_adam(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
                        float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, bool use_multimem, int nblocks, int nthreads,
                        cudaStream_t stream);
+// In-bucket LAMB. The moments of every shard run as launch_multi_tensor_lamb_stage1 over the shard's segments (one parameter ∩ the
+// owned slice each). lamb_ratio: parameter t's local {Σw², Σu²} is the fixed-order sum of the seg_nblk[t] stage-1 partials at
+// seg_ptr[t] (0 blocks: no segment on this rank); the per-rank pairs are exchanged through the symmetric `box`
+// (2 halves · kMaxPeers · nparams double2 at box_off, half = parity) and summed in rank order → ratio[t] (fp32, identical bits on
+// every rank) and sums[t]. shard_lamb: w ← w − lr·r·u on the owned slice, r = ratio[segs[3s+2]] for the elements
+// [segs[3s], segs[3s+1]) of the shard (1 elsewhere, and everywhere when weight_decay == 0), then the weights are all-gathered.
+void launch_lamb_ratio(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const uint64_t* seg_ptr, const int32_t* seg_nblk, int nparams,
+                       uint32_t parity, float* ratio, double* sums, cudaStream_t stream);
+void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, float* master, const float* exp_avg,
+                       const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, const LambParams& hp, bool use_multimem,
+                       int nblocks, int nthreads, cudaStream_t stream);
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,
                          int nblocks, int nthreads, cudaStream_t stream);
 void launch_peer_barrier(const PeerCtx& ctx, cudaStream_t stream);
@@ -188,6 +220,13 @@ void launch_multi_tensor_adam_mp(const TensorListDesc& d, int dtype, const AdamP
 // mixed precision: lists [param(T), grad(T), master(f32)(, momentum(f32) when has_momentum)]
 void launch_multi_tensor_sgd_mp(const TensorListDesc& d, int dtype, bool has_momentum, const SgdParams& hp, float grad_scale,
                                 cudaStream_t stream);
+// LAMB in two launches, lists [param(T), grad(T), exp_avg(f32), exp_avg_sq(f32)(, master(f32) when mixed)]. Stage 1: the moments with
+// g = grad·*coef (coef nullable = 1), fp64 {Σw², Σu²} of each block in sums[2·block], gradient cleared when zero_grad. Stage 2: each
+// block sums its tensor's block partials in a fixed order, forms the trust ratio and applies w ← w − lr·r·u (u recomputed from the
+// new moments); mixed writes the fp32 master and the parameter rounded once.
+void launch_multi_tensor_lamb_stage1(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const float* coef, double* sums, bool zero_grad,
+                                     cudaStream_t stream);
+void launch_multi_tensor_lamb_stage2(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const double* sums, cudaStream_t stream);
 // QAdam momentum pre-step (bagua/torch_api/algorithms/q_adam.py:193-221): m = beta1*m + (1-beta1)*g
 void launch_qadam_momentum(float* exp_avg, const void* grad, int grad_dtype, size_t numel, float beta1, cudaStream_t stream);
 

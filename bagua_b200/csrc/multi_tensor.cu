@@ -11,6 +11,7 @@
 
 #include "dispatch.h"
 #include "kernels.h"
+#include "lamb.cuh"
 #include "quant.cuh"
 
 namespace bagua {
@@ -345,6 +346,112 @@ void launch_multi_tensor_adam(const TensorListDesc& d, int dtype, const AdamPara
         multi_tensor_adam_kernel<T><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, grad_scale);
     });
     check_launch("multi_tensor_adam");
+}
+
+// ---- LAMB: moments + per-block norms, then per-tensor trust ratio + apply ---------------------------------------
+// Stage 1 leaves one fp64 {Σw², Σu²} pair per block (sums[2·block], no atomics); a block belongs to exactly one tensor, so stage 2
+// gets a tensor's norms by adding its blocks' pairs in block order. Stage 2 recomputes u from the new moments and the unchanged w with
+// the same lamb_direction, so no per-element buffer holds u between the launches.
+template <typename T, bool MIXED>
+__global__ void __launch_bounds__(kThreads)
+    multi_tensor_lamb_stage1_kernel(TensorListDesc d, LambParams hp, const float* coef, double* sums, int zero_grad) {
+    __shared__ double s_w[kThreads / 32], s_u[kThreads / 32];
+    const int t = d.block_to_tensor[blockIdx.x];
+    const size_t off = static_cast<size_t>(d.block_to_chunk[blockIdx.x]) * d.chunk;
+    const size_t n = static_cast<size_t>(d.sizes[t]);
+    const size_t len = (n - off) < static_cast<size_t>(d.chunk) ? (n - off) : static_cast<size_t>(d.chunk);
+    const T* p = reinterpret_cast<const T*>(d.ptrs[t]) + off;
+    T* g = reinterpret_cast<T*>(d.ptrs[d.n_tensors + t]) + off;
+    float* m1 = reinterpret_cast<float*>(d.ptrs[2 * d.n_tensors + t]) + off;
+    float* m2 = reinterpret_cast<float*>(d.ptrs[3 * d.n_tensors + t]) + off;
+    const float* mw = MIXED ? reinterpret_cast<const float*>(d.ptrs[4 * d.n_tensors + t]) + off : nullptr;
+    const float c = coef != nullptr ? *coef : 1.f;
+    double sw = 0.0, su = 0.0;
+    for (size_t i = threadIdx.x; i < len; i += blockDim.x) {
+        const float w = MIXED ? mw[i] : to_f32<T>(p[i]);
+        const float gg = coef != nullptr ? __fmul_rn(c, to_f32<T>(g[i])) : to_f32<T>(g[i]);
+        float a = m1[i], b = m2[i];
+        lamb_moments(gg, a, b, hp);
+        const float u = lamb_direction(w, a, b, hp);
+        m1[i] = a;
+        m2[i] = b;
+        if (zero_grad) g[i] = from_f32<T>(0.f);
+        sw += static_cast<double>(w) * static_cast<double>(w);
+        su += static_cast<double>(u) * static_cast<double>(u);
+    }
+    // fixed order: a shuffle tree per warp, then the warps in index order
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        sw += __shfl_xor_sync(0xffffffffu, sw, o);
+        su += __shfl_xor_sync(0xffffffffu, su, o);
+    }
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = sw, s_u[threadIdx.x >> 5] = su;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double a = 0.0, b = 0.0;
+        for (unsigned k = 0; k < blockDim.x / 32; ++k) a += s_w[k], b += s_u[k];
+        sums[2 * blockIdx.x] = a;
+        sums[2 * blockIdx.x + 1] = b;
+    }
+}
+
+template <typename T, bool MIXED>
+__global__ void __launch_bounds__(kThreads) multi_tensor_lamb_stage2_kernel(TensorListDesc d, LambParams hp, const double* sums) {
+    __shared__ float s_ratio;
+    const int t = d.block_to_tensor[blockIdx.x];
+    const int chunk_idx = d.block_to_chunk[blockIdx.x];
+    const size_t off = static_cast<size_t>(chunk_idx) * d.chunk;
+    const size_t n = static_cast<size_t>(d.sizes[t]);
+    const size_t len = (n - off) < static_cast<size_t>(d.chunk) ? (n - off) : static_cast<size_t>(d.chunk);
+    if (threadIdx.x < 32) {  // the tensor's blocks are consecutive from blockIdx.x − chunk_idx: one warp adds their pairs in a fixed order
+        const int first = blockIdx.x - chunk_idx;
+        const int nb = static_cast<int>((n + d.chunk - 1) / d.chunk);
+        double a = 0.0, b = 0.0;
+        for (int k = threadIdx.x; k < nb; k += 32) a += sums[2 * (first + k)], b += sums[2 * (first + k) + 1];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            a += __shfl_xor_sync(0xffffffffu, a, o);
+            b += __shfl_xor_sync(0xffffffffu, b, o);
+        }
+        if (threadIdx.x == 0) s_ratio = lamb_ratio(a, b);
+    }
+    __syncthreads();
+    const float r = s_ratio;
+    T* p = reinterpret_cast<T*>(d.ptrs[t]) + off;
+    const float* m1 = reinterpret_cast<const float*>(d.ptrs[2 * d.n_tensors + t]) + off;
+    const float* m2 = reinterpret_cast<const float*>(d.ptrs[3 * d.n_tensors + t]) + off;
+    float* mw = MIXED ? reinterpret_cast<float*>(d.ptrs[4 * d.n_tensors + t]) + off : nullptr;
+    for (size_t i = threadIdx.x; i < len; i += blockDim.x) {
+        const float w = MIXED ? mw[i] : to_f32<T>(p[i]);
+        const float nw = lamb_apply(w, lamb_direction(w, m1[i], m2[i], hp), r, hp);
+        if (MIXED) mw[i] = nw;
+        p[i] = from_f32<T>(nw);
+    }
+}
+
+void launch_multi_tensor_lamb_stage1(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const float* coef, double* sums, bool zero_grad,
+                                     cudaStream_t stream) {
+    if (d.n_blocks <= 0) return;
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
+        using T = decltype(tag);
+        if (mixed)
+            multi_tensor_lamb_stage1_kernel<T, true><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, coef, sums, zero_grad ? 1 : 0);
+        else
+            multi_tensor_lamb_stage1_kernel<T, false><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, coef, sums, zero_grad ? 1 : 0);
+    });
+    check_launch("multi_tensor_lamb_stage1");
+}
+
+void launch_multi_tensor_lamb_stage2(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const double* sums, cudaStream_t stream) {
+    if (d.n_blocks <= 0) return;
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
+        using T = decltype(tag);
+        if (mixed)
+            multi_tensor_lamb_stage2_kernel<T, true><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, sums);
+        else
+            multi_tensor_lamb_stage2_kernel<T, false><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, sums);
+    });
+    check_launch("multi_tensor_lamb_stage2");
 }
 
 // ---- QAdam momentum pre-step -------------------------------------------------------------------------------------

@@ -208,6 +208,36 @@ void ShardAdamOp::run(Bucket&, StreamHandle stream, int) {
     steps_++;
 }
 
+void LambMomentsOp::run(Bucket&, StreamHandle stream, int) {
+    LambParams hp;
+    {
+        std::lock_guard<std::mutex> lk(mu_);
+        hp = lamb_params(lr_, b1_, b2_, eps_, wd_, steps_ + 1);
+    }
+    launch_multi_tensor_lamb_stage1(desc_, F32, false, hp, reinterpret_cast<const float*>(coef_), reinterpret_cast<double*>(partials_), false, S(stream));
+    steps_++;
+}
+
+void LambRatioOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("lamb_ratio");
+    launch_lamb_ratio(comm_->ctx(), box_.buf, box_off_, reinterpret_cast<const uint64_t*>(seg_ptr_), reinterpret_cast<const int32_t*>(seg_nblk_), nparams_,
+                      static_cast<uint32_t>(calls_ & 1u), reinterpret_cast<float*>(ratio_), reinterpret_cast<double*>(sums_), S(stream));
+    calls_++;
+}
+
+void ShardLambOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("shard_lamb");
+    LambParams hp;
+    {
+        std::lock_guard<std::mutex> lk(mu_);
+        hp = lamb_params(lr_, b1_, b2_, eps_, wd_, steps_ + 1);
+    }
+    launch_shard_lamb(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_), reinterpret_cast<const float*>(m1_),
+                      reinterpret_cast<const float*>(m2_), reinterpret_cast<const int32_t*>(segs_), nsegs_, reinterpret_cast<const float*>(ratio_), hp, use_mc_,
+                      cfg_.nblocks, cfg_.nthreads, S(stream));
+    steps_++;
+}
+
 int PeerAverageOp::shift_one_peer(int rank, int nranks, int64_t step) {
     const int64_t r = rank, n = nranks;
     if (rank < nranks / 2) return static_cast<int>(((step + r) % ((n + 1) / 2)) + (n / 2));

@@ -327,6 +327,85 @@ private:
     std::mutex mu_;
 };
 
+// In-bucket LAMB, run from step() after phase A (ShardGradOp): LambMomentsOp per bucket (the multi-tensor stage-1 kernel over the
+// shard's segment table: fp32 master / gradient shard·*coef / moments, fp64 {Σw², Σu²} per block into `partials`), LambRatioOp once
+// per step (the per-parameter exchange), ShardLambOp per bucket (apply + all-gather + barrier). The moments and apply ops carry the
+// step count (bias corrections) and advance together.
+class LambMomentsOp final : public CommOp {
+public:
+    LambMomentsOp(uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, uint64_t coef, uint64_t partials)
+        : desc_{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes), reinterpret_cast<const int32_t*>(b2t),
+                reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk},
+          coef_(coef), partials_(partials) {}
+    const char* kind() const override { return "lamb_moments"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return false; }  // bias corrections are passed by value
+    void set_hyper(float lr, float beta1, float beta2, float eps, float weight_decay) {
+        std::lock_guard<std::mutex> lk(mu_);
+        lr_ = lr, b1_ = beta1, b2_ = beta2, eps_ = eps, wd_ = weight_decay;
+    }
+    uint64_t steps() const { return steps_; }
+    void set_steps(uint64_t s) { steps_ = s; }
+
+private:
+    TensorListDesc desc_;
+    uint64_t coef_, partials_;
+    float lr_ = 1e-3f, b1_ = 0.9f, b2_ = 0.999f, eps_ = 1e-6f, wd_ = 0.01f;
+    uint64_t steps_ = 0;
+    std::mutex mu_;
+};
+
+class LambRatioOp final : public CommOp {
+public:
+    LambRatioOp(std::shared_ptr<PeerComm> comm, SymmBuf box, size_t box_off, uint64_t seg_ptr, uint64_t seg_nblk, int nparams, uint64_t ratio, uint64_t sums)
+        : comm_(std::move(comm)), box_(box), box_off_(box_off), seg_ptr_(seg_ptr), seg_nblk_(seg_nblk), nparams_(nparams), ratio_(ratio), sums_(sums) {}
+    const char* kind() const override { return "lamb_ratio"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return false; }  // the box half alternates with the call counter
+    uint64_t calls() const { return calls_; }
+    static size_t box_bytes(int nparams) { return 2 * static_cast<size_t>(kMaxPeers) * nparams * 2 * sizeof(double); }
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf box_;
+    size_t box_off_;
+    uint64_t seg_ptr_, seg_nblk_;
+    int nparams_;
+    uint64_t ratio_, sums_;
+    uint64_t calls_ = 0;
+};
+
+class ShardLambOp final : public CommOp {
+public:
+    ShardLambOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t master, uint64_t exp_avg, uint64_t exp_avg_sq,
+                uint64_t segs, int nsegs, uint64_t ratio, bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), master_(master), m1_(exp_avg), m2_(exp_avg_sq), segs_(segs),
+          nsegs_(nsegs), ratio_(ratio), use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return "shard_lamb"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return false; }
+    void set_hyper(float lr, float beta1, float beta2, float eps, float weight_decay) {
+        std::lock_guard<std::mutex> lk(mu_);
+        lr_ = lr, b1_ = beta1, b2_ = beta2, eps_ = eps, wd_ = weight_decay;
+    }
+    uint64_t steps() const { return steps_; }
+    void set_steps(uint64_t s) { steps_ = s; }
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf weights_;
+    size_t w_off_, bytes_;
+    int dtype_;
+    uint64_t master_, m1_, m2_, segs_;
+    int nsegs_;
+    uint64_t ratio_;
+    bool use_mc_;
+    LaunchCfg cfg_;
+    float lr_ = 1e-3f, b1_ = 0.9f, b2_ = 0.999f, eps_ = 1e-6f, wd_ = 0.01f;
+    uint64_t steps_ = 0;
+    std::mutex mu_;
+};
+
 // Decentralized SGD, shift_one pairing (peer formula: comm_ops/decentralized_full_precision_synchronous.rs:81-85).
 class PeerAverageOp final : public CommOp {
 public:

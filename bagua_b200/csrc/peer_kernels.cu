@@ -6,6 +6,7 @@
 // happen in ONE kernel that issues peer (P2P) or NVLS multicast loads/stores itself.
 #include "dispatch.h"
 #include "kernels.h"
+#include "lamb.cuh"
 #include "peer.cuh"
 
 namespace bagua {
@@ -503,6 +504,93 @@ __global__ void __launch_bounds__(512) shard_adam_kernel(PeerCtx ctx, PeerBuf we
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// In-bucket LAMB. Its trust ratio is a norm over a whole parameter, and the owned slices cut parameters anywhere, so after phase A
+// (shard_grad_kernel, unchanged) step() runs: the moments of each shard (multi_tensor_lamb_stage1 over the shard's segments, one
+// parameter ∩ owned slice each, leaving fp64 {Σw², Σu²} per block) → lamb_ratio_kernel, once per step → shard_lamb_kernel per bucket.
+//
+// lamb_ratio_kernel, one CTA: parameter t's local pair is the sum of its segment's block pairs in block order; the pairs go to slot
+// [rank][t] of every peer's box, double-buffered by the op's call counter like grad_norm_kernel (a rank writes a half again two calls
+// later, after every peer has left the call in between), then the barrier, then the P slots in rank order → the same bits everywhere.
+// ---------------------------------------------------------------------------------------------------------
+constexpr int kRatioThreads = 512;
+__global__ void __launch_bounds__(kRatioThreads) lamb_ratio_kernel(PeerCtx ctx, PeerBuf box, size_t box_off, const uint64_t* seg_ptr, const int32_t* seg_nblk,
+                                                                   int nparams, uint32_t parity, float* ratio, double* sums) {
+    const uint32_t e0 = load_epoch(ctx);
+    const size_t half = box_off + static_cast<size_t>(parity & 1u) * kMaxPeers * nparams * 2 * sizeof(double);
+    for (int t = threadIdx.x; t < nparams; t += blockDim.x) {
+        const double* part = reinterpret_cast<const double*>(seg_ptr[t]);
+        double a = 0.0, b = 0.0;
+        for (int k = 0; k < seg_nblk[t]; ++k) a += part[2 * k], b += part[2 * k + 1];
+        const size_t slot = half + (static_cast<size_t>(ctx.rank) * nparams + t) * 2 * sizeof(double);
+        for (int p = 0; p < ctx.world; ++p) {
+            st_peer_f64(box.ptr[p] + slot, a);
+            st_peer_f64(box.ptr[p] + slot + sizeof(double), b);
+        }
+    }
+    const bool ok = peer_barrier(ctx, e0 + 1);
+    const char* mybox = box.ptr[ctx.rank] + half;
+    for (int t = threadIdx.x; t < nparams; t += blockDim.x) {
+        double a = __longlong_as_double(0x7ff8000000000000ll), b = a;
+        if (ok) {
+            a = 0.0, b = 0.0;
+            for (int p = 0; p < ctx.world; ++p) {
+                const char* slot = mybox + (static_cast<size_t>(p) * nparams + t) * 2 * sizeof(double);
+                a += ld_peer_f64(slot);
+                b += ld_peer_f64(slot + sizeof(double));
+            }
+        }
+        ratio[t] = ok ? lamb_ratio(a, b) : __int_as_float(0x7fc00000);
+        sums[2 * t] = a;
+        sums[2 * t + 1] = b;
+    }
+    store_epoch(ctx, e0 + 1);
+}
+
+// segs = [nsegs][lo, hi, param] sorted by lo, disjoint, with gaps where the padding tensor lies. The last segment with lo ≤ e
+// (−1: none), by bisection; the walk below finds it once per vector and advances it element by element, since a 16-byte vector may
+// hold elements of several parameters.
+__device__ __forceinline__ int lamb_segment_at(const int32_t* segs, int nsegs, int64_t e) {
+    int lo = 0, hi = nsegs;  // first segment with lo > e
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (segs[3 * mid] <= e) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo - 1;
+}
+
+// Apply and publish: w ← w − lr·r·u on the owned slice with u recomputed from the stage-1 moments (lamb_direction, the same code
+// that fed Σu²), all-gather of the weights, closing barrier — the walk of shard_adam_kernel over the fp32 master.
+template <typename T, int P, bool USE_MC>
+__global__ void __launch_bounds__(512) shard_lamb_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, float* master, const float* exp_avg,
+                                                         const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, LambParams hp) {
+    const uint32_t e0 = load_epoch(ctx);
+    constexpr int N = Vec16<T>::N;
+    update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), master, [&](size_t j, const float* w0, float* w) {
+        const float4* ap = reinterpret_cast<const float4*>(exp_avg + j * N);
+        const float4* bp = reinterpret_cast<const float4*>(exp_avg_sq + j * N);
+        int s = lamb_segment_at(segs, nsegs, static_cast<int64_t>(j * N));
+#pragma unroll
+        for (int q = 0; q < N / 4; ++q) {
+            const float4 aa = ap[q], bb = bp[q];
+            const float av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int64_t e = static_cast<int64_t>(j * N + 4 * q + k);
+                while (s + 1 < nsegs && segs[3 * (s + 1)] <= e) ++s;
+                const float r = (s >= 0 && e < segs[3 * s + 1]) ? ratio[segs[3 * s + 2]] : 1.f;
+                w[4 * q + k] = lamb_apply(w0[4 * q + k], lamb_direction(w0[4 * q + k], av[k], bv[k], hp), r, hp);
+            }
+        }
+        float4* wp = reinterpret_cast<float4*>(master + j * N);
+#pragma unroll
+        for (int q = 0; q < N / 4; ++q) wp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+    });
+    peer_barrier(ctx, e0 + 1);
+    store_epoch(ctx, e0 + 1);
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // Decentralized SGD, shift_one: out = (mine + peer's weights) / 2, the peer's bucket being read straight over
 // NVLink (replaces grouped send/recv + average kernel, comm_ops/decentralized_full_precision_synchronous.rs:81-92).
 // ---------------------------------------------------------------------------------------------------------
@@ -853,6 +941,30 @@ void launch_shard_adam(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off,
         });
     });
     check_launch("shard_adam");
+}
+
+void launch_lamb_ratio(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const uint64_t* seg_ptr, const int32_t* seg_nblk, int nparams,
+                       uint32_t parity, float* ratio, double* sums, cudaStream_t stream) {
+    if (box_off % 8) throw std::runtime_error("bagua: lamb_ratio box offset must be 8-byte aligned");
+    if (nparams < 1) throw std::runtime_error("bagua: lamb_ratio needs at least one parameter");
+    lamb_ratio_kernel<<<1, kRatioThreads, 0, stream>>>(ctx, box, box_off, seg_ptr, seg_nblk, nparams, parity, ratio, sums);
+    check_launch("lamb_ratio");
+}
+
+void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, float* master, const float* exp_avg,
+                       const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, const LambParams& hp, bool use_multimem,
+                       int nblocks, int nthreads, cudaStream_t stream) {
+    const size_t vecs = peer_vecs("shard_lamb", bytes, w_off, 0, nblocks);
+    if (vecs == 0) return;
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(ctx.world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                shard_lamb_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
+                    ctx, weights, w_off, vecs, master, exp_avg, exp_avg_sq, segs, nsegs, ratio, hp);
+            });
+        });
+    });
+    check_launch("shard_lamb");
 }
 
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,

@@ -16,7 +16,7 @@ import torch
 from ..core import dtype_code, native
 from ..tensor import dense_strides
 
-__all__ = ["FusedSGD", "FusedAdam", "flat_sgd_", "flat_adam_", "multi_tensor_plan"]
+__all__ = ["FusedSGD", "FusedAdam", "FusedLAMB", "flat_sgd_", "flat_adam_", "multi_tensor_plan"]
 
 
 def _stream() -> int:
@@ -517,3 +517,99 @@ class FusedAdam(_FusedBase):
             bc1, bc2 = 1 - b1 ** st["step"], 1 - b2 ** st["step"]
             denom = (st["exp_avg_sq"].sqrt() / (bc2 ** 0.5)).add_(group["eps"])
             p.data.addcdiv_(st["exp_avg"], denom, value=-group["lr"] / bc1)
+
+
+class FusedLAMB(_FusedBase):
+    """LAMB with layer-wise trust ratios, two multi-tensor kernels per (dtype, step count) and step.
+
+    The rule is LAMB (You et al., 2019, "Large Batch Optimization for Deep Learning") with the semantics of apex ``FusedLAMB``
+    at its defaults (bias correction, gradient averaging, decoupled weight decay inside the update, no NVLAMB):
+
+    ``m ← β1·m + (1−β1)·g``, ``v ← β2·v + (1−β2)·g²``, ``u = (m/bc1) / (sqrt(v)/sqrt(bc2) + eps) + wd·w``,
+    ``w ← w − lr·r·u`` with the trust ratio ``r = ‖w‖/‖u‖`` over each whole parameter when ``wd ≠ 0`` and both norms are
+    positive, else 1 — so a no-decay group (biases, LayerNorm) gets no layer adaptation.
+
+    On CUDA every step is two multi-tensor kernels per (dtype, step count): the moments with per-block fp64 ``Σw²``/``Σu²``,
+    then the per-parameter ratio (a fixed-order sum of the parameter's block partials, rounded to fp32 once) and the update.
+    Moments are fp32; ``master_weights=True`` keeps fp32 master weights for bf16/fp16 parameters and writes the parameter
+    rounded once. ``zero_grad_in_step=True`` clears the gradients in the first kernel. CPU tensors take a torch implementation
+    of the same rule."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01, master_weights=True, zero_grad_in_step=True):
+        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
+        super().__init__(params, defaults, master_weights, zero_grad_in_step)
+        self._sums: Dict[tuple, torch.Tensor] = {}
+
+    @torch.no_grad()
+    def step(self, closure=None, only: Optional[set] = None):
+        """``only``: see :meth:`FusedSGD.step`."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        C = native()
+        for gi, group in enumerate(self.param_groups):
+            lr, (b1, b2), eps, wd = group["lr"], group["betas"], group["eps"], group["weight_decay"]
+            params = [p for p in group["params"] if p.grad is not None and (only is None or id(p) in only)]
+            if not params:
+                continue
+            if not _kernels_apply(params):
+                self._torch_step(params, group)
+                continue
+            for p in params:
+                st = self.state[p]
+                if "exp_avg" not in st:
+                    # fp32 moments in the parameter's memory order (the kernels walk raw memory)
+                    st["exp_avg"] = torch.zeros_like(p.data, dtype=torch.float32)
+                    st["exp_avg_sq"] = torch.zeros_like(p.data, dtype=torch.float32)
+                    st["step"] = 0
+                    if self.master_weights and p.dtype in (torch.float16, torch.bfloat16):
+                        st["master"] = torch.empty_like(p.data, dtype=torch.float32).copy_(p.data)
+                st["step"] += 1
+            for (dt, k), ps in _launch_groups(params, lambda p: int(self.state[p]["step"])):
+                mixed = self.master_weights and dt in (torch.float16, torch.bfloat16)
+                step = int(self.state[ps[0]]["step"])
+                grads = [_grad_in_layout(p, dt) for p in ps]
+                lists = [[p.data for p in ps], grads, [self.state[p]["exp_avg"] for p in ps], [self.state[p]["exp_avg_sq"] for p in ps]]
+                if mixed:
+                    lists.append([self.state[p]["master"] for p in ps])
+                plan = _cached_plan(self._multi, (gi, dt, k), lists)
+                sums = self._sums.get((gi, dt, k))
+                if sums is None or sums.shape[0] < plan.n_blocks:
+                    sums = self._sums[(gi, dt, k)] = torch.empty(max(plan.n_blocks, 1), 2, dtype=torch.float64, device=ps[0].device)
+                hyper = (dtype_code(dt), mixed, float(lr), float(b1), float(b2), float(eps), float(wd), step)
+                C.multi_tensor_lamb_stage1(*plan.args(), *hyper, 0, sums.data_ptr(), bool(self.zero_grad_in_step), _stream())
+                C.multi_tensor_lamb_stage2(*plan.args(), *hyper, sums.data_ptr(), _stream())
+                self.kernel_launches += 2
+                if self.zero_grad_in_step:
+                    for p, g in zip(ps, grads):
+                        if g is not p.grad:   # the kernel cleared a converted copy
+                            p.grad.zero_()
+        if only is None:
+            self._grads_zeroed = self.zero_grad_in_step
+        return loss
+
+    def _torch_step(self, params, group):
+        """The same rule in torch fp32 (CPU tensors)."""
+        b1, b2 = group["betas"]
+        eps, wd, lr = group["eps"], group["weight_decay"], group["lr"]
+        for p in params:
+            st = self.state[p]
+            if "exp_avg" not in st:
+                st["exp_avg"] = torch.zeros_like(p.data, dtype=torch.float32)
+                st["exp_avg_sq"] = torch.zeros_like(p.data, dtype=torch.float32)
+                st["step"] = 0
+            st["step"] += 1
+            g = p.grad.float()
+            m, v = st["exp_avg"], st["exp_avg_sq"]
+            m.mul_(b1).add_(g, alpha=1 - b1)
+            v.mul_(b2).addcmul_(g, g, value=1 - b2)
+            bc1, bc2 = 1 - b1 ** st["step"], 1 - b2 ** st["step"]
+            w = p.data.float()
+            u = (m / bc1) / (v.sqrt() / bc2 ** 0.5 + eps) + wd * w
+            r = 1.0
+            if wd != 0:
+                wn, un = float(w.double().norm()), float(u.double().norm())
+                if wn > 0 and un > 0:
+                    r = float(torch.tensor(wn / un, dtype=torch.float32))
+            p.data.copy_(w - (lr * r) * u)

@@ -53,7 +53,7 @@ class GradientAllReduceAlgorithm(Algorithm):
 # ---------------------------------------------------------------------------------------------------------------
 # Checkpointable state of the in-bucket optimizers
 # ---------------------------------------------------------------------------------------------------------------
-_STATE_KEYS = {"sgd": ("master", "momentum_buffer"), "adam": ("master", "exp_avg", "exp_avg_sq")}
+_STATE_KEYS = {"sgd": ("master", "momentum_buffer"), "adam": ("master", "exp_avg", "exp_avg_sq"), "lamb": ("master", "exp_avg", "exp_avg_sq")}
 
 
 def consolidate_shards(shards, numel: int, layout):
@@ -139,7 +139,8 @@ class _ShardedStateMixin:
         for key, t in zip(_STATE_KEYS[self._kind], rec["state"]):
             per_name = {name: st[key] for name, st in sd["state"].items() if key in st}
             t.copy_(shard_of(per_name, rec["layout"], rec["numel"], rec["lo"], rec["hi"], t.numel(), device=t.device))
-        rec["op"].set_steps(int(sd.get("steps", 0)))
+        for op in rec.get("step_ops", (rec["op"],)):   # LAMB: its moments op carries the bias corrections as well
+            op.set_steps(int(sd.get("steps", 0)))
 
     def refresh_master_weights(self):
         """Re-read the fp32 master shards from the model weights (call after loading or editing weights without optimizer
@@ -345,6 +346,79 @@ def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weigh
     return opt
 
 
+class ShardedFusedLamb(object):
+    """Marker mix-in: see :func:`make_sharded_fused_lamb`."""
+
+
+def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01, max_grad_norm=None):
+    """LAMB (apex ``FusedLAMB`` semantics, see :class:`bagua_b200.ops.optim.FusedLAMB`) on the in-bucket sharded path: each rank
+    keeps fp32 master weights and both moments for its 1/N slice of every bucket.
+
+    The trust ratio ``‖w‖/‖u‖`` is a norm over a whole parameter, and a bucket's slices cut parameters anywhere, so the update
+    cannot run during backward: each bucket kernel only reduce-scatters the averaged gradient into an fp32 shard (4 bytes per
+    element / N), and ``step()`` then runs, on the current stream: the norm exchange when ``max_grad_norm`` is set (as for
+    :func:`make_sharded_fused_sgd`), the moments of every shard with fp64 partial ``Σw²``/``Σu²`` per parameter segment, one
+    exchange of the per-parameter sums between the ranks (every rank obtains the same fp32 ratios), and the update plus the
+    all-gather of the weights per bucket. A parameter group with ``weight_decay=0`` gets no layer adaptation (ratio 1). With one
+    process, or without a peer engine, it behaves like :class:`bagua_b200.ops.optim.FusedLAMB`; see ``docs/algorithms.md``."""
+    from ...ops.optim import FusedLAMB
+
+    class _ShardedFusedLamb(_ShardedStateMixin, FusedLAMB, ShardedFusedLamb):
+        _kind = "lamb"
+
+        def __init__(self, *a, **k):
+            super().__init__(*a, **k)
+            self._comm_ops = []      # the apply op of every bucket (ShardLambOp), in bucket order
+            self._lamb_moments = []  # the moments op of every bucket (LambMomentsOp), same order
+            self._lamb = None        # the per-parameter ratio exchange shared by all buckets (see _lamb_state)
+            self._shards = []
+
+        def _sync_hyper(self):
+            groups = getattr(self, "_comm_groups", ())
+            for i, op in enumerate(self._comm_ops):
+                g = self.param_groups[groups[i] if i < len(groups) else 0]
+                hyper = (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]))
+                op.set_hyper(*hyper)
+                self._lamb_moments[i].set_hyper(*hyper)
+
+        def step(self, closure=None):
+            """The norm exchange (with ``max_grad_norm``, unless ``clip_grad_norm_`` ran it), the moments of every bucket's shard,
+            the ratio exchange, the update and all-gather of every bucket, then the parameters outside the buckets with the same
+            clipping coefficient — ``2·buckets + 1`` launches (+1 with clipping), all on the current stream, no host
+            synchronisation. The ordering argument of :meth:`_ShardedStateMixin.step` applies unchanged."""
+            if not self._comm_ops:
+                return super().step(closure)
+            import torch
+
+            from ...core import native
+
+            self._sync_hyper()
+            coef = None
+            if getattr(self, "_clip", None) is not None:
+                if not getattr(self, "_norm_pending", False):
+                    self._launch_norm(self.max_grad_norm)
+                self._norm_pending = False
+                coef = self._clip["out"][1]
+            lam = self._lamb
+            if lam["ratio_op"] is None:
+                raise RuntimeError("the LAMB ratio exchange was not built: not every bucket of the model has been initialised")
+            dev = lam["ratio"].device
+            C, stream = native(), torch.cuda.current_stream(dev).cuda_stream
+            for op in self._lamb_moments:
+                C.run_op(op, stream, dev.index)
+            C.run_op(lam["ratio_op"], stream, dev.index)
+            for op in self._comm_ops:
+                C.run_op(op, stream, dev.index)
+            self.kernel_launches += 2 * len(self._comm_ops) + 1
+            self._step_uncovered(coef)
+            self._grads_zeroed = True
+            return None
+
+    opt = _ShardedFusedLamb(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, master_weights=True, zero_grad_in_step=True)
+    opt.max_grad_norm = _check_bound(max_grad_norm)
+    return opt
+
+
 class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
     def __init__(self, process_group, optimizer, average: bool = True):
         super().__init__(process_group, hierarchical=False, average=average)
@@ -384,6 +458,9 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         opt._covered = set()
         opt._uncovered_cache = None
         opt._clip = None
+        if isinstance(opt, ShardedFusedLamb):
+            opt._lamb_moments = []
+            opt._lamb = None
 
     def tensors_to_buckets(self, tensors, do_flatten):
         from ...bucket import BaguaBucket
@@ -442,7 +519,8 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         eng = bucket._engine(self.process_group)
         opt = self.optimizer
         is_adam = isinstance(opt, ShardedFusedAdam)
-        if eng is None or bucket._slice is None or not (isinstance(opt, ShardedFusedSGD) or is_adam):
+        is_lamb = isinstance(opt, ShardedFusedLamb)
+        if eng is None or bucket._slice is None or not (isinstance(opt, ShardedFusedSGD) or is_adam or is_lamb):
             return super().init_operations(bagua_ddp, bucket)
         group_index = getattr(bucket, "_fused_group", 0)
         C = native()
@@ -487,10 +565,16 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         cfg = eng.launch_cfg("multimem" if use_mc else "two_shot", nbytes, blocks=int(os.environ.get("BAGUA_FUSED_BLOCKS", "0")) or (16 if use_mc else 64))
         scale = (1.0 / n) if self.average else 1.0
         code = dtype_code(flat.dtype)
-        second = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device) if is_adam else None
-        bucket._fused_state = (master, momentum, second) if is_adam else (master, momentum)
+        second = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device) if is_adam or is_lamb else None
+        bucket._fused_state = (master, momentum, second) if is_adam or is_lamb else (master, momentum)
         clip = opt.max_grad_norm is not None
-        if clip:
+        layout = [(t.bagua_tensor_name, (t.bagua_getter_closure().data_ptr() - base) // flat.element_size(), t.bagua_getter_closure().numel(),
+                   tuple(t.shape), tuple(dense_strides(t))) for t in bucket.tensors if not t.bagua_tensor_name.startswith("bagua_padding_tensor")]
+        step_ops = None
+        if is_lamb:
+            op, moments = self._lamb_ops(eng, bagua_ddp, bucket, wslice, nbytes, code, lo, hi, layout, scale, use_mc, cfg)
+            step_ops = (op, moments)
+        elif clip:
             # phase A in the bucket program (reduce-scatter into the fp32 shard + per-CTA Σx²); the update op runs in step()
             st = opt._clip if getattr(opt, "_clip", None) is not None else self._clip_state(eng, bagua_ddp, bucket, flat.device)
             shard = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
@@ -512,19 +596,103 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         else:
             op = C.AllReduceSgdOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                   master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
-        if not clip:
+        if not (clip or is_lamb):
             bucket.backend_bucket.append_op(op)
         bucket._ops_keepalive.append(op)
-        bucket.allreduce_variant = ("fused_adam_" if is_adam else "fused_sgd_") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
+        kind = "fused_lamb_" if is_lamb else ("fused_adam_" if is_adam else "fused_sgd_")
+        bucket.allreduce_variant = kind + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
         opt._comm_ops.append(op)
         if not hasattr(opt, "_comm_groups"):
             opt._comm_groups = []
         opt._comm_groups.append(group_index)
-        layout = [(t.bagua_tensor_name, (t.bagua_getter_closure().data_ptr() - base) // flat.element_size(), t.bagua_getter_closure().numel(),
-                   tuple(t.shape), tuple(dense_strides(t))) for t in bucket.tensors if not t.bagua_tensor_name.startswith("bagua_padding_tensor")]
-        opt._register_shard({"bucket": bucket.name, "group": self.process_group, "numel": flat.numel(), "lo": lo, "hi": hi, "layout": layout,
-                             "state": bucket._fused_state, "op": op, "weights": wflat, "param_ids": [id(t) for t in bucket.tensors]})
+        rec = {"bucket": bucket.name, "group": self.process_group, "numel": flat.numel(), "lo": lo, "hi": hi, "layout": layout,
+               "state": bucket._fused_state, "op": op, "weights": wflat, "param_ids": [id(t) for t in bucket.tensors]}
+        if step_ops is not None:
+            rec["step_ops"] = step_ops
+        opt._register_shard(rec)
         opt._sync_hyper()
+
+    def _lamb_state(self, eng, bagua_ddp, bucket, device):
+        """State of the LAMB ratio exchange, shared by all buckets: a global index of the bucketed parameters (bucket order,
+        padding excluded), the per-parameter outputs (fp32 ratio, fp64 {Σw², Σu²}), the stage-1 partial tables filled in bucket by
+        bucket, the phase-A partial sums when no norm exchange provides them, and the symmetric box (2 halves × MAX_PEERS ×
+        parameters × 2 doubles, freed with the first bucket's other symmetric slices when the buckets are rebuilt)."""
+        import torch
+
+        from ...core import native
+
+        C = native()
+        names = [t.bagua_tensor_name for b in bagua_ddp.bagua_buckets for t in b.tensors if not t.bagua_tensor_name.startswith("bagua_padding_tensor")]
+        box = eng.alloc(C.LambRatioOp.box_bytes(len(names)))
+        bucket._companion_slices.append(box)
+        lam = {"index": {n: i for i, n in enumerate(names)}, "pending": set(names), "box": box,
+               "ratio": torch.ones(len(names), dtype=torch.float32, device=device),
+               "sums": torch.zeros(len(names), 2, dtype=torch.float64, device=device),
+               "seg_ptr": [0] * len(names), "seg_nblk": [0] * len(names), "ratio_op": None,
+               "partials": torch.zeros(len(bagua_ddp.bagua_buckets), C.MAX_COMM_BLOCKS, dtype=torch.float64, device=device)}
+        self.optimizer._lamb = lam
+        return lam
+
+    def _lamb_ops(self, eng, bagua_ddp, bucket, wslice, nbytes, code, lo, hi, layout, scale, use_mc, cfg):
+        """One bucket of the in-bucket LAMB: phase A (ShardGradOp) in the bucket program; the moments op over the shard's segments
+        (parameter ∩ [lo, hi), shard-local offsets), whose per-block partials the ratio exchange sums per parameter; the apply op.
+        The ratio exchange is built once every bucketed parameter has its table entry."""
+        import torch
+
+        from ...core import native
+        from ...ops.optim import multi_tensor_plan
+
+        C = native()
+        opt = self.optimizer
+        master, m1, m2 = bucket._fused_state
+        dev = master.device
+        lam = opt._lamb if opt._lamb is not None else self._lamb_state(eng, bagua_ddp, bucket, dev)
+        row_index = [b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)
+        shard = torch.zeros_like(master)
+        bucket._clip_shard = shard
+        coef_ptr = 0
+        if opt.max_grad_norm is not None:
+            st = opt._clip if getattr(opt, "_clip", None) is not None else self._clip_state(eng, bagua_ddp, bucket, dev)
+            row = st["partials"][row_index]
+            coef_ptr = st["out"][1:].data_ptr()
+        else:
+            row = lam["partials"][row_index]   # phase A writes its Σx² partials somewhere; nothing reads them without clipping
+        red = C.ShardGradOp(eng.comm, bucket._slice.buf, bucket._slice.offset, nbytes, code, shard.data_ptr(), row.data_ptr(), scale, True, use_mc, cfg)
+        bucket.backend_bucket.append_op(red)
+        segs, views = [], [[], [], [], []]
+        for name, off, n, _, _ in layout:
+            a, b = max(off, lo), min(off + n, hi)
+            if a < b:
+                segs.append((a - lo, b - lo, lam["index"][name]))
+                for lst, buf in zip(views, (master, shard, m1, m2)):
+                    lst.append(buf[a - lo: b - lo])
+        if segs:
+            plan = multi_tensor_plan(views)
+            partials = torch.zeros(max(plan.n_blocks, 1), 2, dtype=torch.float64, device=dev)
+            moments = C.LambMomentsOp(*plan.args(), coef_ptr, partials.data_ptr())
+            blk = 0
+            for a, b, t in segs:   # the plan gives each segment ceil(len / CHUNK) consecutive blocks, in segment order
+                nb = (b - a + plan.CHUNK - 1) // plan.CHUNK
+                lam["seg_ptr"][t], lam["seg_nblk"][t] = partials.data_ptr() + 16 * blk, nb
+                blk += nb
+            assert blk == plan.n_blocks
+        else:   # an empty slice (small bucket, many ranks): no moments to update, but the rank still takes part in every exchange
+            plan, partials = None, torch.zeros(1, 2, dtype=torch.float64, device=dev)
+            moments = C.LambMomentsOp(0, 0, 0, 0, 0, 0, 65536, coef_ptr, partials.data_ptr())
+        table = torch.tensor([v for s in segs for v in s] or [0, 0, 0], dtype=torch.int32, device=dev)
+        op = C.ShardLambOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, master.data_ptr(), m1.data_ptr(), m2.data_ptr(), table.data_ptr(), len(segs),
+                           lam["ratio"].data_ptr(), use_mc, cfg)
+        bucket._ops_keepalive += [red, moments]
+        bucket._lamb_tables = (plan, partials, table, segs)
+        opt._lamb_moments.append(moments)
+        lam["pending"] -= {name for name, *_ in layout}
+        if not lam["pending"]:
+            ptrs = torch.tensor(lam["seg_ptr"], dtype=torch.int64, device=dev)
+            nblk = torch.tensor(lam["seg_nblk"], dtype=torch.int32, device=dev)
+            lam["tables"] = (ptrs, nblk)
+            lam["ratio_op"] = C.LambRatioOp(eng.comm, lam["box"].buf, lam["box"].offset, ptrs.data_ptr(), nblk.data_ptr(), len(lam["index"]),
+                                            lam["ratio"].data_ptr(), lam["sums"].data_ptr())
+        return op, moments
 
 
 class FusedGradientAllReduceAlgorithm(Algorithm):

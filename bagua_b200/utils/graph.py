@@ -29,12 +29,14 @@ __all__ = ["GraphedTrainStep", "graph_safe_optimizer"]
 
 def graph_safe_optimizer(opt: torch.optim.Optimizer) -> Optional[str]:
     """``None`` when ``opt`` may run inside a captured graph, else the reason it may not."""
-    from ..ops.optim import FusedAdam, FusedSGD
+    from ..ops.optim import FusedAdam, FusedLAMB, FusedSGD
 
     if isinstance(opt, FusedSGD):
         return None
     if isinstance(opt, FusedAdam):
         return "FusedAdam passes the step count to its kernel by value (bias correction changes every step)"
+    if isinstance(opt, FusedLAMB):
+        return "FusedLAMB passes the step count to its kernels by value (bias correction changes every step)"
     if isinstance(opt, torch.optim.SGD):
         return None
     if all(g.get("capturable", False) for g in opt.param_groups):
@@ -57,6 +59,9 @@ class GraphedTrainStep:
             if getattr(opt, "_comm_ops", None) is not None and getattr(opt, "max_grad_norm", None) is not None:
                 raise NotImplementedError("a sharded fused optimizer with max_grad_norm runs its norm exchange and clipped update from "
                                           "step() with per-call host state (box parity, step count); it cannot be captured in a CUDA graph")
+            if getattr(opt, "_comm_ops", None) is not None and getattr(opt, "_kind", None) == "lamb":
+                raise NotImplementedError("the sharded fused LAMB optimizer runs its moments, ratio exchange and update from step() with "
+                                          "per-call host state (box parity, step count); it cannot be captured in a CUDA graph")
             why = graph_safe_optimizer(opt)
             if why is not None:
                 raise ValueError(f"optimizer cannot be captured in a CUDA graph: {why}")

@@ -17,7 +17,7 @@ import torch  # noqa: E402
 
 from bagua_b200.core import dtype_code, native  # noqa: E402
 from bagua_b200.ops import gemm, quant  # noqa: E402
-from bagua_b200.ops.optim import flat_adam_, flat_sgd_  # noqa: E402
+from bagua_b200.ops.optim import flat_adam_, flat_sgd_, multi_tensor_plan  # noqa: E402
 from bagua_b200.parallel.virtual import VirtualPeerWorld  # noqa: E402
 
 from bench import ClockSampler  # noqa: E402
@@ -109,6 +109,26 @@ gate = C.WeightGate(0)
 snap, avg = w.alloc(NB), w.alloc(NB)
 aa = C.AsyncAverageOp(comm, out.data_ptr(), snap.buf, 0, avg.buf, 0, NB, code, gate, 1.0, False, w.cfg(16))
 timed("async_average_kernel<bf16,P=1,peer> 64MiB", lambda: run(aa), 8 * NB)
+# in-bucket LAMB on the 64 MiB bucket as ONE parameter (shard, master, moments fp32)
+shard = torch.randn(n, device=dev)
+lplan = multi_tensor_plan([[master], [shard], [mom], [m2]])
+lpart = torch.zeros(lplan.n_blocks, 2, dtype=torch.float64, device=dev)
+lmom = C.LambMomentsOp(*lplan.args(), 0, lpart.data_ptr())
+lmom.set_hyper(1e-3, 0.9, 0.999, 1e-6, 0.01)
+# reads master, shard, both moments (16B); writes both moments (8B) per element
+timed("multi_tensor_lamb_stage1_kernel<f32> 32M-element shard (in-bucket moments)", lambda: run(lmom), n * 24)
+lptr = torch.tensor([lpart.data_ptr()], dtype=torch.int64, device=dev)
+lnb = torch.tensor([lplan.n_blocks], dtype=torch.int32, device=dev)
+lratio, lsums = torch.ones(1, device=dev), torch.zeros(1, 2, dtype=torch.float64, device=dev)
+rbox = w.alloc(C.LambRatioOp.box_bytes(1))
+lrop = C.LambRatioOp(comm, rbox.buf, 0, lptr.data_ptr(), lnb.data_ptr(), 1, lratio.data_ptr(), lsums.data_ptr())
+timed("lamb_ratio_kernel 1 parameter", lambda: run(lrop), lplan.n_blocks * 16)
+lsegs = torch.tensor([0, n, 0], dtype=torch.int32, device=dev)
+lapply = C.ShardLambOp(comm, b.buf, 0, NB, code, master.data_ptr(), mom.data_ptr(), m2.data_ptr(), lsegs.data_ptr(), 1, lratio.data_ptr(), False, w.cfg(32))
+lapply.set_hyper(1e-3, 0.9, 0.999, 1e-6, 0.01)
+# reads master and both moments (12B); writes master (4B) + weights (2B) per element
+timed("shard_lamb_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(lapply), n * 18)
+del shard, lpart
 
 # single-GPU kernels ------------------------------------------------------------------------------------------------------
 P = 138 * 1000 * 1000 // 8 * 8   # VGG16-sized arena
