@@ -43,6 +43,12 @@ AdamParams make_adam(float lr, float b1, float b2, float eps, float wd, int step
     p.amsgrad = 0;
     return p;
 }
+
+// set_hyper(<the rule's hyper-parameters in Hyper's field order>), steps() and set_steps(n) of an optimizer op.
+template <class Op, class... Args>
+void def_stepped(py::class_<Op, CommOp, std::shared_ptr<Op>>& cls) {
+    cls.def("set_hyper", [](Op& op, Args... args) { op.set_hyper({args...}); }).def("steps", &Op::steps).def("set_steps", &Op::set_steps);
+}
 }  // namespace
 
 // Entry point for the optional torch extension (csrc/torch_hooks): marks a tensor ready without going through Python.
@@ -224,31 +230,25 @@ PYBIND11_MODULE(_C, m) {
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, uint64_t, uint64_t, size_t, int, float, LaunchCfg>(), py::arg("comm"),
              py::arg("staging"), py::arg("staging_off"), py::arg("slot_bytes"), py::arg("in_ptr"), py::arg("out_ptr"), py::arg("bytes"), py::arg("dtype"),
              py::arg("scale"), py::arg("cfg"));
-    py::class_<AllReduceSgdOp, CommOp, std::shared_ptr<AllReduceSgdOp>>(m, "AllReduceSgdOp")
-        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, SymmBuf, size_t, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool,
-                      LaunchCfg>(),
-             py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"),
-             py::arg("master_ptr"), py::arg("momentum_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg"))
-        .def("set_hyper", &AllReduceSgdOp::set_hyper)
-        .def("set_grad_scale", &AllReduceSgdOp::set_grad_scale)
-        .def("steps", &AllReduceSgdOp::steps)
-        .def("set_steps", &AllReduceSgdOp::set_steps);
+    def_stepped<AllReduceSgdOp, float, float, float, float, bool>(
+        py::class_<AllReduceSgdOp, CommOp, std::shared_ptr<AllReduceSgdOp>>(m, "AllReduceSgdOp")
+            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, SymmBuf, size_t, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool,
+                          LaunchCfg>(),
+                 py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"),
+                 py::arg("master_ptr"), py::arg("momentum_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg")));
     py::class_<ReduceScatterOp, CommOp, std::shared_ptr<ReduceScatterOp>>(m, "ReduceScatterOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, float, bool, LaunchCfg>(), py::arg("comm"), py::arg("buf"), py::arg("off"),
              py::arg("bytes"), py::arg("dtype"), py::arg("scale"), py::arg("use_multimem"), py::arg("cfg"));
     py::class_<AllGatherOp, CommOp, std::shared_ptr<AllGatherOp>>(m, "AllGatherOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, bool, LaunchCfg>(), py::arg("comm"), py::arg("buf"), py::arg("off"),
              py::arg("bytes"), py::arg("dtype"), py::arg("use_multimem"), py::arg("cfg"));
-    py::class_<AllReduceAdamOp, CommOp, std::shared_ptr<AllReduceAdamOp>>(m, "AllReduceAdamOp")
-        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, SymmBuf, size_t, size_t, size_t, int, uint64_t, uint64_t, uint64_t, float, bool, bool,
-                      LaunchCfg>(),
-             py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"),
-             py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"),
-             py::arg("cfg"))
-        .def("set_hyper", &AllReduceAdamOp::set_hyper)
-        .def("set_grad_scale", &AllReduceAdamOp::set_grad_scale)
-        .def("steps", &AllReduceAdamOp::steps)
-        .def("set_steps", &AllReduceAdamOp::set_steps);
+    def_stepped<AllReduceAdamOp, float, float, float, float, float, bool>(
+        py::class_<AllReduceAdamOp, CommOp, std::shared_ptr<AllReduceAdamOp>>(m, "AllReduceAdamOp")
+            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, SymmBuf, size_t, size_t, size_t, int, uint64_t, uint64_t, uint64_t, float, bool, bool,
+                          LaunchCfg>(),
+                 py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"),
+                 py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"),
+                 py::arg("cfg")));
     py::class_<ShardGradOp, CommOp, std::shared_ptr<ShardGradOp>>(m, "ShardGradOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool, LaunchCfg>(), py::arg("comm"),
              py::arg("grads"), py::arg("g_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("partials_ptr"), py::arg("scale"),
@@ -258,38 +258,30 @@ PYBIND11_MODULE(_C, m) {
              py::arg("partials_ptr"), py::arg("nslots"), py::arg("extra_ptr"), py::arg("out_ptr"))
         .def("set_max_norm", &GradNormOp::set_max_norm)
         .def("calls", &GradNormOp::calls);
-    py::class_<ShardSgdOp, CommOp, std::shared_ptr<ShardSgdOp>>(m, "ShardSgdOp")
-        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(), py::arg("comm"),
-             py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"), py::arg("master_ptr"),
-             py::arg("momentum_ptr"), py::arg("use_multimem"), py::arg("cfg"))
-        .def("set_hyper", &ShardSgdOp::set_hyper)
-        .def("steps", &ShardSgdOp::steps)
-        .def("set_steps", &ShardSgdOp::set_steps);
-    py::class_<ShardAdamOp, CommOp, std::shared_ptr<ShardAdamOp>>(m, "ShardAdamOp")
-        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(),
-             py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
-             py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("use_multimem"), py::arg("cfg"))
-        .def("set_hyper", &ShardAdamOp::set_hyper)
-        .def("steps", &ShardAdamOp::steps)
-        .def("set_steps", &ShardAdamOp::set_steps);
-    py::class_<LambMomentsOp, CommOp, std::shared_ptr<LambMomentsOp>>(m, "LambMomentsOp")
-        .def(py::init<uint64_t, uint64_t, uint64_t, uint64_t, int, int, int, uint64_t, uint64_t>(), py::arg("ptrs"), py::arg("sizes"), py::arg("b2t"),
-             py::arg("b2c"), py::arg("n_tensors"), py::arg("n_blocks"), py::arg("chunk"), py::arg("coef_ptr"), py::arg("partials_ptr"))
-        .def("set_hyper", &LambMomentsOp::set_hyper)
-        .def("steps", &LambMomentsOp::steps)
-        .def("set_steps", &LambMomentsOp::set_steps);
+    def_stepped<ShardSgdOp, float, float, float, float, bool>(
+        py::class_<ShardSgdOp, CommOp, std::shared_ptr<ShardSgdOp>>(m, "ShardSgdOp")
+            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(), py::arg("comm"),
+                 py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"), py::arg("master_ptr"),
+                 py::arg("momentum_ptr"), py::arg("use_multimem"), py::arg("cfg")));
+    def_stepped<ShardAdamOp, float, float, float, float, float, bool>(
+        py::class_<ShardAdamOp, CommOp, std::shared_ptr<ShardAdamOp>>(m, "ShardAdamOp")
+            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(),
+                 py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
+                 py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("use_multimem"), py::arg("cfg")));
+    def_stepped<LambMomentsOp, float, float, float, float, float>(
+        py::class_<LambMomentsOp, CommOp, std::shared_ptr<LambMomentsOp>>(m, "LambMomentsOp")
+            .def(py::init<uint64_t, uint64_t, uint64_t, uint64_t, int, int, int, uint64_t, uint64_t>(), py::arg("ptrs"), py::arg("sizes"), py::arg("b2t"),
+                 py::arg("b2c"), py::arg("n_tensors"), py::arg("n_blocks"), py::arg("chunk"), py::arg("coef_ptr"), py::arg("partials_ptr")));
     py::class_<LambRatioOp, CommOp, std::shared_ptr<LambRatioOp>>(m, "LambRatioOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, uint64_t, uint64_t, int, uint64_t, uint64_t>(), py::arg("comm"), py::arg("box"),
              py::arg("box_off"), py::arg("seg_ptr"), py::arg("seg_nblk"), py::arg("nparams"), py::arg("ratio_ptr"), py::arg("sums_ptr"))
         .def("calls", &LambRatioOp::calls)
         .def_static("box_bytes", &LambRatioOp::box_bytes);
-    py::class_<ShardLambOp, CommOp, std::shared_ptr<ShardLambOp>>(m, "ShardLambOp")
-        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, int, uint64_t, bool, LaunchCfg>(),
-             py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("master_ptr"), py::arg("exp_avg_ptr"),
-             py::arg("exp_avg_sq_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("ratio_ptr"), py::arg("use_multimem"), py::arg("cfg"))
-        .def("set_hyper", &ShardLambOp::set_hyper)
-        .def("steps", &ShardLambOp::steps)
-        .def("set_steps", &ShardLambOp::set_steps);
+    def_stepped<ShardLambOp, float, float, float, float, float>(
+        py::class_<ShardLambOp, CommOp, std::shared_ptr<ShardLambOp>>(m, "ShardLambOp")
+            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, int, uint64_t, bool, LaunchCfg>(),
+                 py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("master_ptr"), py::arg("exp_avg_ptr"),
+                 py::arg("exp_avg_sq_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("ratio_ptr"), py::arg("use_multimem"), py::arg("cfg")));
     py::class_<PeerAverageOp, CommOp, std::shared_ptr<PeerAverageOp>>(m, "PeerAverageOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, uint64_t, size_t, int, LaunchCfg>(), py::arg("comm"), py::arg("weights"),
              py::arg("off"), py::arg("out_ptr"), py::arg("bytes"), py::arg("dtype"), py::arg("cfg"))

@@ -46,12 +46,17 @@ struct LambParams {
     float bias_correction2;  // 1 - beta2^t
 };
 
+// 1 - beta^step of the in-bucket Adam and LAMB ops and of FusedLAMB: in double, rounded once.
+inline float bias_correction(float beta, uint64_t step) {
+    return static_cast<float>(1.0 - std::pow(static_cast<double>(beta), static_cast<double>(step)));
+}
+
+inline AdamParams adam_params(float lr, float beta1, float beta2, float eps, float weight_decay, bool adamw, uint64_t step) {
+    return AdamParams{lr, beta1, beta2, eps, weight_decay, bias_correction(beta1, step), bias_correction(beta2, step), adamw ? 1 : 0, 0};
+}
+
 inline LambParams lamb_params(float lr, float beta1, float beta2, float eps, float weight_decay, uint64_t step) {
-    LambParams p{lr, beta1, beta2, eps, weight_decay, 0.f, 0.f};
-    const double t = static_cast<double>(step);  // as the in-bucket Adam ops compute them: in double, rounded once
-    p.bias_correction1 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta1), t));
-    p.bias_correction2 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta2), t));
-    return p;
+    return LambParams{lr, beta1, beta2, eps, weight_decay, bias_correction(beta1, step), bias_correction(beta2, step)};
 }
 
 // ---- peer kernels (peer_kernels.cu) ------------------------------------------------------------------------

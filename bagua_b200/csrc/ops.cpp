@@ -1,7 +1,5 @@
 #include "ops.h"
 
-#include <cmath>
-
 #include <cuda_runtime.h>
 
 #include <cstring>
@@ -125,16 +123,8 @@ void AllReduceOneShotOp::run(Bucket&, StreamHandle stream, int) {
 
 void AllReduceSgdOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("allreduce_sgd");
-    SgdParams hp;
-    float scale;
-    {
-        std::lock_guard<std::mutex> lk(mu_);
-        hp = hp_;
-        scale = scale_;
-    }
-    hp.first_step = steps_ == 0 ? 1 : 0;
     launch_allreduce_sgd(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_),
-                         reinterpret_cast<float*>(momentum_), hp, scale, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
+                         reinterpret_cast<float*>(momentum_), params(), scale_, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
     steps_++;
 }
 
@@ -150,18 +140,8 @@ void AllGatherOp::run(Bucket&, StreamHandle stream, int) {
 
 void AllReduceAdamOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("allreduce_adam");
-    AdamParams hp{};
-    float scale;
-    {
-        std::lock_guard<std::mutex> lk(mu_);
-        hp.lr = lr_, hp.beta1 = b1_, hp.beta2 = b2_, hp.eps = eps_, hp.weight_decay = wd_, hp.adamw = adamw_ ? 1 : 0;
-        scale = scale_;
-    }
-    const double t = static_cast<double>(steps_ + 1);
-    hp.bias_correction1 = static_cast<float>(1.0 - std::pow(static_cast<double>(hp.beta1), t));
-    hp.bias_correction2 = static_cast<float>(1.0 - std::pow(static_cast<double>(hp.beta2), t));
     launch_allreduce_adam(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_),
-                          reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), hp, scale, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads,
+                          reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), params(), scale_, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads,
                           S(stream));
     steps_++;
 }
@@ -181,40 +161,21 @@ void GradNormOp::run(Bucket&, StreamHandle stream, int) {
 
 void ShardSgdOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("shard_sgd");
-    SgdParams hp;
-    {
-        std::lock_guard<std::mutex> lk(mu_);
-        hp = hp_;
-    }
-    hp.first_step = steps_ == 0 ? 1 : 0;
     launch_shard_sgd(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), reinterpret_cast<const float*>(coef_),
-                     reinterpret_cast<float*>(master_), reinterpret_cast<float*>(momentum_), hp, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
+                     reinterpret_cast<float*>(master_), reinterpret_cast<float*>(momentum_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
     steps_++;
 }
 
 void ShardAdamOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("shard_adam");
-    AdamParams hp{};
-    {
-        std::lock_guard<std::mutex> lk(mu_);
-        hp.lr = lr_, hp.beta1 = b1_, hp.beta2 = b2_, hp.eps = eps_, hp.weight_decay = wd_, hp.adamw = adamw_ ? 1 : 0;
-    }
-    const double t = static_cast<double>(steps_ + 1);
-    hp.bias_correction1 = static_cast<float>(1.0 - std::pow(static_cast<double>(hp.beta1), t));
-    hp.bias_correction2 = static_cast<float>(1.0 - std::pow(static_cast<double>(hp.beta2), t));
     launch_shard_adam(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), reinterpret_cast<const float*>(coef_),
-                      reinterpret_cast<float*>(master_), reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), hp, use_mc_, cfg_.nblocks, cfg_.nthreads,
+                      reinterpret_cast<float*>(master_), reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads,
                       S(stream));
     steps_++;
 }
 
 void LambMomentsOp::run(Bucket&, StreamHandle stream, int) {
-    LambParams hp;
-    {
-        std::lock_guard<std::mutex> lk(mu_);
-        hp = lamb_params(lr_, b1_, b2_, eps_, wd_, steps_ + 1);
-    }
-    launch_multi_tensor_lamb_stage1(desc_, F32, false, hp, reinterpret_cast<const float*>(coef_), reinterpret_cast<double*>(partials_), false, S(stream));
+    launch_multi_tensor_lamb_stage1(desc_, F32, false, params(), reinterpret_cast<const float*>(coef_), reinterpret_cast<double*>(partials_), false, S(stream));
     steps_++;
 }
 
@@ -227,13 +188,8 @@ void LambRatioOp::run(Bucket&, StreamHandle stream, int) {
 
 void ShardLambOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("shard_lamb");
-    LambParams hp;
-    {
-        std::lock_guard<std::mutex> lk(mu_);
-        hp = lamb_params(lr_, b1_, b2_, eps_, wd_, steps_ + 1);
-    }
     launch_shard_lamb(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_), reinterpret_cast<const float*>(m1_),
-                      reinterpret_cast<const float*>(m2_), reinterpret_cast<const int32_t*>(segs_), nsegs_, reinterpret_cast<const float*>(ratio_), hp, use_mc_,
+                      reinterpret_cast<const float*>(m2_), reinterpret_cast<const int32_t*>(segs_), nsegs_, reinterpret_cast<const float*>(ratio_), params(), use_mc_,
                       cfg_.nblocks, cfg_.nthreads, S(stream));
     steps_++;
 }

@@ -115,8 +115,54 @@ private:
     LaunchCfg cfg_;
 };
 
+// Host hyper-parameters of the in-bucket optimizer rules, in the argument order of their ops' set_hyper.
+struct SgdHyper {
+    float lr = 0.01f, momentum = 0.f, dampening = 0.f, weight_decay = 0.f;
+    bool nesterov = false;
+};
+struct AdamHyper {
+    float lr = 1e-3f, beta1 = 0.9f, beta2 = 0.999f, eps = 1e-8f, weight_decay = 0.f;
+    bool adamw = false;
+};
+struct LambHyper {
+    float lr = 1e-3f, beta1 = 0.9f, beta2 = 0.999f, eps = 1e-6f, weight_decay = 0.01f;
+};
+
+// What a rule's kernel receives at the launch that follows `steps` earlier ones.
+inline SgdParams device_params(const SgdHyper& h, uint64_t steps) {
+    return SgdParams{h.lr, h.momentum, h.dampening, h.weight_decay, h.nesterov ? 1 : 0, steps == 0 ? 1 : 0};
+}
+inline AdamParams device_params(const AdamHyper& h, uint64_t steps) {
+    return adam_params(h.lr, h.beta1, h.beta2, h.eps, h.weight_decay, h.adamw, steps + 1);
+}
+inline LambParams device_params(const LambHyper& h, uint64_t steps) { return lamb_params(h.lr, h.beta1, h.beta2, h.eps, h.weight_decay, steps + 1); }
+
+// An optimizer op: hyper-parameters published from Python (the forward pre-hook may do so while the comm worker runs the op, hence
+// the lock) and the count of launches so far, which checkpoints save and restore.
+template <class Hyper>
+class SteppedOp : public CommOp {
+public:
+    void set_hyper(const Hyper& h) {
+        std::lock_guard<std::mutex> lk(mu_);
+        hp_ = h;
+    }
+    uint64_t steps() const { return steps_; }
+    void set_steps(uint64_t s) { steps_ = s; }
+
+protected:
+    auto params() {
+        std::lock_guard<std::mutex> lk(mu_);
+        return device_params(hp_, steps_);
+    }
+    uint64_t steps_ = 0;
+
+private:
+    Hyper hp_;
+    std::mutex mu_;
+};
+
 // reduce-scatter(grads) → SGD on the owned shard → all-gather(weights), one kernel per bucket.
-class AllReduceSgdOp final : public CommOp {
+class AllReduceSgdOp final : public SteppedOp<SgdHyper> {
 public:
     AllReduceSgdOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, SymmBuf weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
                    uint64_t master, uint64_t momentum, float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg)
@@ -125,16 +171,6 @@ public:
     const char* kind() const override { return "allreduce_sgd"; }
     void run(Bucket&, StreamHandle stream, int device) override;
     bool step_invariant() const override { return steps_ > 0; }  // only the very first launch differs (momentum initialisation)
-    void set_hyper(float lr, float momentum, float dampening, float weight_decay, bool nesterov) {
-        std::lock_guard<std::mutex> lk(mu_);
-        hp_.lr = lr, hp_.momentum = momentum, hp_.dampening = dampening, hp_.weight_decay = weight_decay, hp_.nesterov = nesterov;
-    }
-    void set_grad_scale(float s) {
-        std::lock_guard<std::mutex> lk(mu_);
-        scale_ = s;
-    }
-    uint64_t steps() const { return steps_; }
-    void set_steps(uint64_t s) { steps_ = s; }
 
 private:
     std::shared_ptr<PeerComm> comm_;
@@ -142,12 +178,9 @@ private:
     size_t g_off_, w_off_, bytes_;
     int dtype_;
     uint64_t master_, momentum_;
-    float scale_;
+    const float scale_;
     bool zero_grads_, use_mc_;
     LaunchCfg cfg_;
-    SgdParams hp_{0.01f, 0.f, 0.f, 0.f, 0, 1};
-    uint64_t steps_ = 0;
-    std::mutex mu_;
 };
 
 // Intra-node halves of a hierarchical all-reduce (see reduce_scatter_kernel): ReduceScatterOp, then a callback op that
@@ -186,7 +219,7 @@ private:
 };
 
 // The Adam / AdamW flavour of the fused bucket op; the step counter (bias correction) advances with every launch.
-class AllReduceAdamOp final : public CommOp {
+class AllReduceAdamOp final : public SteppedOp<AdamHyper> {
 public:
     AllReduceAdamOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, SymmBuf weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
                     uint64_t master, uint64_t exp_avg, uint64_t exp_avg_sq, float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg)
@@ -195,16 +228,6 @@ public:
     const char* kind() const override { return "allreduce_adam"; }
     void run(Bucket&, StreamHandle stream, int device) override;
     bool step_invariant() const override { return false; }  // bias corrections are passed by value
-    void set_hyper(float lr, float beta1, float beta2, float eps, float weight_decay, bool adamw) {
-        std::lock_guard<std::mutex> lk(mu_);
-        lr_ = lr, b1_ = beta1, b2_ = beta2, eps_ = eps, wd_ = weight_decay, adamw_ = adamw;
-    }
-    void set_grad_scale(float s) {
-        std::lock_guard<std::mutex> lk(mu_);
-        scale_ = s;
-    }
-    uint64_t steps() const { return steps_; }
-    void set_steps(uint64_t s) { steps_ = s; }
 
 private:
     std::shared_ptr<PeerComm> comm_;
@@ -212,13 +235,9 @@ private:
     size_t g_off_, w_off_, bytes_;
     int dtype_;
     uint64_t master_, m1_, m2_;
-    float scale_;
+    const float scale_;
     bool zero_grads_, use_mc_;
     LaunchCfg cfg_;
-    float lr_ = 1e-3f, b1_ = 0.9f, b2_ = 0.999f, eps_ = 1e-8f, wd_ = 0.f;
-    bool adamw_ = false;
-    uint64_t steps_ = 0;
-    std::mutex mu_;
 };
 
 // Global-norm clipping of the in-bucket optimizers (see shard_grad_kernel). Phase A, in the bucket program: reduce-scatter of the
@@ -268,7 +287,7 @@ private:
 
 // Phase B: SGD on the owned shard with the gradient shard·coef, all-gather of the weights. Carries the step counter like
 // AllReduceSgdOp (checkpoints see the same interface).
-class ShardSgdOp final : public CommOp {
+class ShardSgdOp final : public SteppedOp<SgdHyper> {
 public:
     ShardSgdOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
                uint64_t momentum, bool use_multimem, LaunchCfg cfg)
@@ -277,12 +296,6 @@ public:
     const char* kind() const override { return "shard_sgd"; }
     void run(Bucket&, StreamHandle stream, int device) override;
     bool step_invariant() const override { return steps_ > 0; }
-    void set_hyper(float lr, float momentum, float dampening, float weight_decay, bool nesterov) {
-        std::lock_guard<std::mutex> lk(mu_);
-        hp_.lr = lr, hp_.momentum = momentum, hp_.dampening = dampening, hp_.weight_decay = weight_decay, hp_.nesterov = nesterov;
-    }
-    uint64_t steps() const { return steps_; }
-    void set_steps(uint64_t s) { steps_ = s; }
 
 private:
     std::shared_ptr<PeerComm> comm_;
@@ -292,12 +305,9 @@ private:
     uint64_t shard_, coef_, master_, momentum_;
     bool use_mc_;
     LaunchCfg cfg_;
-    SgdParams hp_{0.01f, 0.f, 0.f, 0.f, 0, 1};
-    uint64_t steps_ = 0;
-    std::mutex mu_;
 };
 
-class ShardAdamOp final : public CommOp {
+class ShardAdamOp final : public SteppedOp<AdamHyper> {
 public:
     ShardAdamOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
                 uint64_t exp_avg, uint64_t exp_avg_sq, bool use_multimem, LaunchCfg cfg)
@@ -306,12 +316,6 @@ public:
     const char* kind() const override { return "shard_adam"; }
     void run(Bucket&, StreamHandle stream, int device) override;
     bool step_invariant() const override { return false; }
-    void set_hyper(float lr, float beta1, float beta2, float eps, float weight_decay, bool adamw) {
-        std::lock_guard<std::mutex> lk(mu_);
-        lr_ = lr, b1_ = beta1, b2_ = beta2, eps_ = eps, wd_ = weight_decay, adamw_ = adamw;
-    }
-    uint64_t steps() const { return steps_; }
-    void set_steps(uint64_t s) { steps_ = s; }
 
 private:
     std::shared_ptr<PeerComm> comm_;
@@ -321,17 +325,13 @@ private:
     uint64_t shard_, coef_, master_, m1_, m2_;
     bool use_mc_;
     LaunchCfg cfg_;
-    float lr_ = 1e-3f, b1_ = 0.9f, b2_ = 0.999f, eps_ = 1e-8f, wd_ = 0.f;
-    bool adamw_ = false;
-    uint64_t steps_ = 0;
-    std::mutex mu_;
 };
 
 // In-bucket LAMB, run from step() after phase A (ShardGradOp): LambMomentsOp per bucket (the multi-tensor stage-1 kernel over the
 // shard's segment table: fp32 master / gradient shard·*coef / moments, fp64 {Σw², Σu²} per block into `partials`), LambRatioOp once
 // per step (the per-parameter exchange), ShardLambOp per bucket (apply + all-gather + barrier). The moments and apply ops carry the
 // step count (bias corrections) and advance together.
-class LambMomentsOp final : public CommOp {
+class LambMomentsOp final : public SteppedOp<LambHyper> {
 public:
     LambMomentsOp(uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, uint64_t coef, uint64_t partials)
         : desc_{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes), reinterpret_cast<const int32_t*>(b2t),
@@ -340,19 +340,10 @@ public:
     const char* kind() const override { return "lamb_moments"; }
     void run(Bucket&, StreamHandle stream, int device) override;
     bool step_invariant() const override { return false; }  // bias corrections are passed by value
-    void set_hyper(float lr, float beta1, float beta2, float eps, float weight_decay) {
-        std::lock_guard<std::mutex> lk(mu_);
-        lr_ = lr, b1_ = beta1, b2_ = beta2, eps_ = eps, wd_ = weight_decay;
-    }
-    uint64_t steps() const { return steps_; }
-    void set_steps(uint64_t s) { steps_ = s; }
 
 private:
     TensorListDesc desc_;
     uint64_t coef_, partials_;
-    float lr_ = 1e-3f, b1_ = 0.9f, b2_ = 0.999f, eps_ = 1e-6f, wd_ = 0.01f;
-    uint64_t steps_ = 0;
-    std::mutex mu_;
 };
 
 class LambRatioOp final : public CommOp {
@@ -375,7 +366,7 @@ private:
     uint64_t calls_ = 0;
 };
 
-class ShardLambOp final : public CommOp {
+class ShardLambOp final : public SteppedOp<LambHyper> {
 public:
     ShardLambOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t master, uint64_t exp_avg, uint64_t exp_avg_sq,
                 uint64_t segs, int nsegs, uint64_t ratio, bool use_multimem, LaunchCfg cfg)
@@ -384,12 +375,6 @@ public:
     const char* kind() const override { return "shard_lamb"; }
     void run(Bucket&, StreamHandle stream, int device) override;
     bool step_invariant() const override { return false; }
-    void set_hyper(float lr, float beta1, float beta2, float eps, float weight_decay) {
-        std::lock_guard<std::mutex> lk(mu_);
-        lr_ = lr, b1_ = beta1, b2_ = beta2, eps_ = eps, wd_ = weight_decay;
-    }
-    uint64_t steps() const { return steps_; }
-    void set_steps(uint64_t s) { steps_ = s; }
 
 private:
     std::shared_ptr<PeerComm> comm_;
@@ -401,9 +386,6 @@ private:
     uint64_t ratio_;
     bool use_mc_;
     LaunchCfg cfg_;
-    float lr_ = 1e-3f, b1_ = 0.9f, b2_ = 0.999f, eps_ = 1e-6f, wd_ = 0.01f;
-    uint64_t steps_ = 0;
-    std::mutex mu_;
 };
 
 // Decentralized SGD, shift_one pairing (peer formula: comm_ops/decentralized_full_precision_synchronous.rs:81-85).

@@ -54,6 +54,10 @@ class GradientAllReduceAlgorithm(Algorithm):
 # Checkpointable state of the in-bucket optimizers
 # ---------------------------------------------------------------------------------------------------------------
 _STATE_KEYS = {"sgd": ("master", "momentum_buffer"), "adam": ("master", "exp_avg", "exp_avg_sq"), "lamb": ("master", "exp_avg", "exp_avg_sq")}
+# what set_hyper of a rule's bucket ops takes, from a parameter group (a LAMB bucket's moments and apply op take the same)
+_HYPER = {"sgd": lambda g: (float(g["lr"]), float(g["momentum"]), float(g["dampening"]), float(g["weight_decay"]), bool(g["nesterov"])),
+          "adam": lambda g: (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]), bool(g["adamw"])),
+          "lamb": lambda g: (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]))}
 
 
 def consolidate_shards(shards, numel: int, layout):
@@ -83,6 +87,25 @@ def shard_of(per_name, layout, numel: int, lo: int, hi: int, length: int, device
     return out
 
 
+class _Bucketing:
+    """What an in-bucket optimizer holds for one bucketing of the model. ``FusedGradientAllReduceAlgorithm`` replaces it as a whole
+    whenever the buckets are (re-)built; with no peer engine it stays empty and the optimizer takes the flat path."""
+
+    def __init__(self):
+        self.shards = []       # one record per bucket, see FusedGradientAllReduceAlgorithmImpl.init_operations
+        self.hyper_ops = []    # (op, parameter-group index) of every op that takes hyper-parameters
+        self.covered = set()   # ids of the bucketed parameters
+        self.uncovered = None  # the parameters outside the buckets, looked up once
+        self.clip = None       # the norm exchange shared by all buckets (max_grad_norm), see _clip_state
+        self.lamb = None       # the per-parameter ratio exchange shared by all buckets (LAMB), see _lamb_state
+        # the program step() runs after the norm exchange, on the current stream of `device`: every bucket's pre-update op (LAMB
+        # moments), LAMB's ratio exchange, every bucket's update op; empty when the updates run in the bucket kernels
+        self.pre_ops = []
+        self.update_ops = []
+        self.device = None
+        self.launches = 0      # optimizer-update kernels per step, in the bucket programs or in step()
+
+
 class _ShardedStateMixin:
     """``state_dict()`` / ``load_state_dict()`` of the optimizers whose state lives in 1/N shards next to the buckets.
 
@@ -93,9 +116,23 @@ class _ShardedStateMixin:
     _kind = "sgd"
     max_grad_norm = None
 
+    def __init__(self, *a, **k):
+        super().__init__(*a, **k)
+        self._bucketing = _Bucketing()
+        self._pending_state = None   # a checkpoint loaded while no shard exists, applied bucket by bucket by _register_shard
+        self._norm_pending = False   # clip_grad_norm_ has computed this step's norm
+        self._last_norm = None
+
     @property
     def collective_state_dict(self) -> bool:
-        return bool(getattr(self, "_shards", None))
+        return bool(self._bucketing.shards)
+
+    @property
+    def native_ops_in_step(self) -> bool:
+        """Whether ``step()`` runs native kernels once the bucket kernels are live: the norm exchange and the clipped update with
+        ``max_grad_norm``, LAMB's moments, ratio exchange and update always. They carry per-call host state (box parity, step
+        count), so such a step cannot be captured in a CUDA graph."""
+        return self.max_grad_norm is not None or self._kind == "lamb"
 
     def _gather(self, t, group):
         import torch
@@ -106,15 +143,15 @@ class _ShardedStateMixin:
         return out
 
     def state_dict(self):
-        if not getattr(self, "_shards", None):
+        if not self._bucketing.shards:
             return super().state_dict()
         state = {}
         steps = 0
-        for rec in self._shards:
+        for rec in self._bucketing.shards:
             for key, t in zip(_STATE_KEYS[self._kind], rec["state"]):
                 for name, full in consolidate_shards(self._gather(t, rec["group"]), rec["numel"], rec["layout"]).items():
                     state.setdefault(name, {})[key] = full.cpu()
-            steps = max(steps, int(rec["op"].steps()))
+            steps = max(steps, int(rec["step_ops"][0].steps()))
         groups = [{k: v for k, v in g.items() if k != "params"} for g in self.param_groups]
         # parameters outside the buckets (MoE experts, ignored ones) are stepped by the base class: their state in torch's format
         return {"sharded_fused": self._kind, "steps": steps, "state": state, "param_groups": groups, "uncovered": super().state_dict()}
@@ -128,10 +165,10 @@ class _ShardedStateMixin:
             super().load_state_dict(sd["uncovered"])
         for g, saved in zip(self.param_groups, sd["param_groups"]):
             g.update(saved)
-        if not getattr(self, "_shards", None):
+        if not self._bucketing.shards:
             self._pending_state = sd          # applied bucket by bucket when the algorithm builds the ops (with_bagua)
             return
-        for rec in self._shards:
+        for rec in self._bucketing.shards:
             self._apply_to_shard(rec, sd)
         self._sync_hyper()
 
@@ -139,25 +176,29 @@ class _ShardedStateMixin:
         for key, t in zip(_STATE_KEYS[self._kind], rec["state"]):
             per_name = {name: st[key] for name, st in sd["state"].items() if key in st}
             t.copy_(shard_of(per_name, rec["layout"], rec["numel"], rec["lo"], rec["hi"], t.numel(), device=t.device))
-        for op in rec.get("step_ops", (rec["op"],)):   # LAMB: its moments op carries the bias corrections as well
+        for op in rec["step_ops"]:
             op.set_steps(int(sd.get("steps", 0)))
 
     def refresh_master_weights(self):
         """Re-read the fp32 master shards from the model weights (call after loading or editing weights without optimizer
         state: the next bucket kernel writes ``master − lr·update`` over the parameters)."""
-        if not getattr(self, "_shards", None):
+        if not self._bucketing.shards:
             return super().refresh_master_weights() if hasattr(super(), "refresh_master_weights") else None
-        for rec in self._shards:
+        for rec in self._bucketing.shards:
             lo, hi = rec["lo"], min(rec["hi"], rec["numel"])
             if hi > lo:
                 rec["state"][0][: hi - lo].copy_(rec["weights"][lo:hi].float())
 
+    def _sync_hyper(self):
+        hyper = _HYPER[self._kind]
+        for op, group_index in self._bucketing.hyper_ops:
+            op.set_hyper(*hyper(self.param_groups[group_index]))
+
     def _uncovered(self):
-        candidates = getattr(self, "_uncovered_cache", None)
-        if candidates is None:  # the parameter list is static between (re-)initialisations: looked up once, usually empty
-            covered = getattr(self, "_covered", set())
-            candidates = self._uncovered_cache = [p for g in self.param_groups for p in g["params"] if id(p) not in covered]
-        return [p for p in candidates if p.grad is not None]
+        b = self._bucketing
+        if b.uncovered is None:  # the parameter list is static between (re-)initialisations: looked up once, usually empty
+            b.uncovered = [p for g in self.param_groups for p in g["params"] if id(p) not in b.covered]
+        return [p for p in b.uncovered if p.grad is not None]
 
     def _step_uncovered(self, coef=None):
         """Parameters that no bucket kernel updates — MoE experts (excluded from data parallelism), ignored parameters —
@@ -177,7 +218,7 @@ class _ShardedStateMixin:
     def last_grad_norm(self):
         """Global L2 norm of the averaged gradient at the last step that clipped: a device fp32 0-d tensor with the same bits on
         every rank, overwritten by the next step (no host synchronisation). ``None`` before the first one."""
-        return getattr(self, "_last_norm", None)
+        return self._last_norm
 
     def clip_grad_norm_(self, max_norm: float, norm_type: float = 2.0):
         """Clip by the global L2 norm of the averaged gradient with bound ``max_norm`` for this step and return the norm (device
@@ -187,14 +228,14 @@ class _ShardedStateMixin:
         ``max_grad_norm``: the call then computes the norm that the following ``step()`` applies (``step()`` computes it itself
         when this is not called). Without a peer engine the gradients are ordinary all-reduced tensors and the flat path clips
         them in place."""
-        live = bool(getattr(self, "_comm_ops", None))
+        live = bool(self._bucketing.hyper_ops)
         if float(norm_type) != 2.0 and (live or self.max_grad_norm is not None):
             raise ValueError(f"the sharded fused optimizers clip by the L2 norm only, got norm_type={norm_type}")
         if not live:
             total = super().clip_grad_norm_(max_norm, norm_type)
             self._norm_pending, self._last_norm = True, total
             return total
-        if getattr(self, "_clip", None) is None:
+        if self._bucketing.clip is None:
             raise RuntimeError("the in-bucket optimizer applied this step's update during backward, so its gradients cannot be clipped "
                                "afterwards; construct it with max_grad_norm=... (make_sharded_fused_sgd / make_sharded_fused_adam) to clip "
                                "on this path")
@@ -205,7 +246,7 @@ class _ShardedStateMixin:
 
         from ...core import native
 
-        clip = self._clip
+        clip = self._bucketing.clip
         loose = [p.grad for p in self._uncovered()]
         if loose:   # each rank adds the local Σx² of its parameters outside the buckets: every expert counts once in the total
             clip["extra"].copy_(torch.stack([torch.linalg.vector_norm(g, dtype=torch.float64) for g in loose]).square().sum())
@@ -222,50 +263,54 @@ class _ShardedStateMixin:
         return self._last_norm
 
     def step(self, closure=None):
-        """Without clipping the update already ran in the bucket kernels of this iteration's backward: publish the
-        hyper-parameters for the next one and step the parameters outside the buckets. With ``max_grad_norm``: the norm
-        exchange (unless ``clip_grad_norm_`` ran it), then the clipped update of every bucket's shard and the all-gather of the
-        weights, then the parameters outside the buckets, all on the current stream."""
-        if not self._comm_ops:
-            if self.max_grad_norm is not None and not getattr(self, "_norm_pending", False):
+        """Without a peer engine: the flat optimizer (clipping first with ``max_grad_norm``). Otherwise: publish the
+        hyper-parameters; with ``max_grad_norm`` run the norm exchange (unless ``clip_grad_norm_`` ran it); run the step program
+        of the bucketing on the current stream (see :class:`_Bucketing`; empty when the bucket kernels of this iteration's backward
+        already applied the update); then step the parameters outside the buckets, their gradients scaled by the clipping
+        coefficient. No host synchronisation."""
+        b = self._bucketing
+        if not b.hyper_ops:
+            if self.max_grad_norm is not None and not self._norm_pending:
                 self._last_norm = super().clip_grad_norm_(self.max_grad_norm)
             self._norm_pending = False
             return super().step(closure)
         self._sync_hyper()
         coef = None
-        if getattr(self, "_clip", None) is not None:
+        if b.clip is not None:
+            if not self._norm_pending:
+                self._launch_norm(self.max_grad_norm)
+            self._norm_pending = False
+            coef = b.clip["out"][1]
+        if b.update_ops:
             # Ordering: the post-backward hook made this stream wait for the comm stream, so every phase-A bucket kernel (shard +
             # partials) has finished; the next iteration's bucket launches wait for ready events recorded after this step() on
-            # this stream. So phase A, the norm exchange and phase B of one PeerComm stay totally ordered, the shards and the
+            # this stream. So phase A, the exchanges and the updates of one PeerComm stay totally ordered, the shards and the
             # partials are never overwritten while read, and the weights are all-gathered before the next forward reads them.
             import torch
 
             from ...core import native
 
-            if not getattr(self, "_norm_pending", False):
-                self._launch_norm(self.max_grad_norm)
-            self._norm_pending = False
-            dev = self._clip["out"].device
-            C, stream = native(), torch.cuda.current_stream(dev).cuda_stream
-            for op in self._comm_ops:
-                C.run_op(op, stream, dev.index)
-            coef = self._clip["out"][1]
+            if b.lamb is not None and b.lamb["ratio_op"] is None:
+                raise RuntimeError("the LAMB ratio exchange was not built: not every bucket of the model has been initialised")
+            C, stream, dev = native(), torch.cuda.current_stream(b.device).cuda_stream, b.device.index
+            for op in b.pre_ops:
+                C.run_op(op, stream, dev)
+            if b.lamb is not None:
+                C.run_op(b.lamb["ratio_op"], stream, dev)
+            for op in b.update_ops:
+                C.run_op(op, stream, dev)
         self._step_uncovered(coef)
         self._grads_zeroed = True
-        self.kernel_launches += len(self._comm_ops)
+        self.kernel_launches += b.launches
         return None
 
     def _register_shard(self, rec):
-        if not hasattr(self, "_shards"):
-            self._shards = []
-        if not hasattr(self, "_covered"):
-            self._covered = set()
-        self._covered.update(rec.get("param_ids", ()))
-        self._uncovered_cache = None
-        self._shards.append(rec)
-        pending = getattr(self, "_pending_state", None)
-        if pending is not None:
-            self._apply_to_shard(rec, pending)
+        b = self._bucketing
+        b.covered.update(rec.get("param_ids", ()))
+        b.uncovered = None
+        b.shards.append(rec)
+        if self._pending_state is not None:
+            self._apply_to_shard(rec, self._pending_state)
 
 
 
@@ -298,17 +343,6 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
     class _ShardedFusedSGD(_ShardedStateMixin, FusedSGD, ShardedFusedSGD):
         _kind = "sgd"
 
-        def __init__(self, *a, **k):
-            super().__init__(*a, **k)
-            self._comm_ops = []   # the update op of every bucket (AllReduceSgdOp, or ShardSgdOp when clipping) once the algorithm has taken over
-            self._shards = []
-
-        def _sync_hyper(self):
-            groups = getattr(self, "_comm_groups", ())
-            for i, op in enumerate(self._comm_ops):
-                g = self.param_groups[groups[i] if i < len(groups) else 0]   # every bucket op serves one parameter group
-                op.set_hyper(float(g["lr"]), float(g["momentum"]), float(g["dampening"]), float(g["weight_decay"]), bool(g["nesterov"]))
-
     opt = _ShardedFusedSGD(params, lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
                            master_weights=True, zero_grad_in_step=True)
     opt.max_grad_norm = _check_bound(max_grad_norm)
@@ -329,17 +363,6 @@ def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weigh
     class _ShardedFusedAdam(_ShardedStateMixin, FusedAdam, ShardedFusedAdam):
         _kind = "adam"
 
-        def __init__(self, *a, **k):
-            super().__init__(*a, **k)
-            self._comm_ops = []
-            self._shards = []
-
-        def _sync_hyper(self):
-            groups = getattr(self, "_comm_groups", ())
-            for i, op in enumerate(self._comm_ops):
-                g = self.param_groups[groups[i] if i < len(groups) else 0]
-                op.set_hyper(float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]), bool(g["adamw"]))
-
     opt = _ShardedFusedAdam(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, adamw=adamw, master_weights=True,
                             zero_grad_in_step=True)
     opt.max_grad_norm = _check_bound(max_grad_norm)
@@ -359,60 +382,13 @@ def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weigh
     element / N), and ``step()`` then runs, on the current stream: the norm exchange when ``max_grad_norm`` is set (as for
     :func:`make_sharded_fused_sgd`), the moments of every shard with fp64 partial ``Σw²``/``Σu²`` per parameter segment, one
     exchange of the per-parameter sums between the ranks (every rank obtains the same fp32 ratios), and the update plus the
-    all-gather of the weights per bucket. A parameter group with ``weight_decay=0`` gets no layer adaptation (ratio 1). With one
-    process, or without a peer engine, it behaves like :class:`bagua_b200.ops.optim.FusedLAMB`; see ``docs/algorithms.md``."""
+    all-gather of the weights per bucket — ``2·buckets + 1`` launches (+1 with clipping). A parameter group with
+    ``weight_decay=0`` gets no layer adaptation (ratio 1). With one process, or without a peer engine, it behaves like
+    :class:`bagua_b200.ops.optim.FusedLAMB`; see ``docs/algorithms.md``."""
     from ...ops.optim import FusedLAMB
 
     class _ShardedFusedLamb(_ShardedStateMixin, FusedLAMB, ShardedFusedLamb):
         _kind = "lamb"
-
-        def __init__(self, *a, **k):
-            super().__init__(*a, **k)
-            self._comm_ops = []      # the apply op of every bucket (ShardLambOp), in bucket order
-            self._lamb_moments = []  # the moments op of every bucket (LambMomentsOp), same order
-            self._lamb = None        # the per-parameter ratio exchange shared by all buckets (see _lamb_state)
-            self._shards = []
-
-        def _sync_hyper(self):
-            groups = getattr(self, "_comm_groups", ())
-            for i, op in enumerate(self._comm_ops):
-                g = self.param_groups[groups[i] if i < len(groups) else 0]
-                hyper = (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]))
-                op.set_hyper(*hyper)
-                self._lamb_moments[i].set_hyper(*hyper)
-
-        def step(self, closure=None):
-            """The norm exchange (with ``max_grad_norm``, unless ``clip_grad_norm_`` ran it), the moments of every bucket's shard,
-            the ratio exchange, the update and all-gather of every bucket, then the parameters outside the buckets with the same
-            clipping coefficient — ``2·buckets + 1`` launches (+1 with clipping), all on the current stream, no host
-            synchronisation. The ordering argument of :meth:`_ShardedStateMixin.step` applies unchanged."""
-            if not self._comm_ops:
-                return super().step(closure)
-            import torch
-
-            from ...core import native
-
-            self._sync_hyper()
-            coef = None
-            if getattr(self, "_clip", None) is not None:
-                if not getattr(self, "_norm_pending", False):
-                    self._launch_norm(self.max_grad_norm)
-                self._norm_pending = False
-                coef = self._clip["out"][1]
-            lam = self._lamb
-            if lam["ratio_op"] is None:
-                raise RuntimeError("the LAMB ratio exchange was not built: not every bucket of the model has been initialised")
-            dev = lam["ratio"].device
-            C, stream = native(), torch.cuda.current_stream(dev).cuda_stream
-            for op in self._lamb_moments:
-                C.run_op(op, stream, dev.index)
-            C.run_op(lam["ratio_op"], stream, dev.index)
-            for op in self._comm_ops:
-                C.run_op(op, stream, dev.index)
-            self.kernel_launches += 2 * len(self._comm_ops) + 1
-            self._step_uncovered(coef)
-            self._grads_zeroed = True
-            return None
 
     opt = _ShardedFusedLamb(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, master_weights=True, zero_grad_in_step=True)
     opt.max_grad_norm = _check_bound(max_grad_norm)
@@ -434,9 +410,10 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         called — so the hyper-parameters are published at the start of every iteration (after any ``lr_scheduler.step()`` of
         the previous one), not only from ``step()``."""
         opt = self.optimizer
+        sharded = isinstance(opt, _ShardedStateMixin)
 
         def hook(input):
-            if getattr(opt, "_comm_ops", None):
+            if sharded and opt._bucketing.hyper_ops:
                 opt._sync_hyper()
 
         # _reset_buckets builds this hook after the last init_operations: every new shard has consumed the carried-over state
@@ -447,20 +424,14 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
     def _carry_state_over(self):
         """Called at the start of every (re-)bucketing — with_bagua, the autotune service moving bucket boundaries every 100 steps,
         the find_unused_parameters rebuild: snapshot the sharded master weights / moments / step count in their consolidated
-        (world-size and bucketing independent) form and forget the old shards; ``init_operations`` re-shards from the snapshot.
+        (world-size and bucketing independent) form and forget the old bucketing; ``init_operations`` re-shards from the snapshot.
         Collective (an all-gather per state tensor), like re-bucketing itself."""
         opt = self.optimizer
-        if getattr(opt, "_shards", None):
+        if not isinstance(opt, _ShardedStateMixin):
+            return
+        if opt._bucketing.shards:
             opt._pending_state = opt.state_dict()
-        opt._comm_ops = []
-        opt._comm_groups = []
-        opt._shards = []
-        opt._covered = set()
-        opt._uncovered_cache = None
-        opt._clip = None
-        if isinstance(opt, ShardedFusedLamb):
-            opt._lamb_moments = []
-            opt._lamb = None
+        opt._bucketing = _Bucketing()
 
     def tensors_to_buckets(self, tensors, do_flatten):
         from ...bucket import BaguaBucket
@@ -504,7 +475,6 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         st["box"] = box
         st["norm_op"] = C.GradNormOp(eng.comm, box.buf, box.offset, st["partials"].data_ptr(), st["partials"].numel(), st["extra"].data_ptr(),
                                      st["out"].data_ptr())
-        self.optimizer._clip = st
         return st
 
     def init_operations(self, bagua_ddp, bucket):
@@ -522,6 +492,7 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         is_lamb = isinstance(opt, ShardedFusedLamb)
         if eng is None or bucket._slice is None or not (isinstance(opt, ShardedFusedSGD) or is_adam or is_lamb):
             return super().init_operations(bagua_ddp, bucket)
+        bk = opt._bucketing
         group_index = getattr(bucket, "_fused_group", 0)
         C = native()
         flat = bucket.backend_tensor
@@ -566,49 +537,50 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         scale = (1.0 / n) if self.average else 1.0
         code = dtype_code(flat.dtype)
         second = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device) if is_adam or is_lamb else None
-        bucket._fused_state = (master, momentum, second) if is_adam or is_lamb else (master, momentum)
         clip = opt.max_grad_norm is not None
         layout = [(t.bagua_tensor_name, (t.bagua_getter_closure().data_ptr() - base) // flat.element_size(), t.bagua_getter_closure().numel(),
                    tuple(t.shape), tuple(dense_strides(t))) for t in bucket.tensors if not t.bagua_tensor_name.startswith("bagua_padding_tensor")]
-        step_ops = None
-        if is_lamb:
-            op, moments = self._lamb_ops(eng, bagua_ddp, bucket, wslice, nbytes, code, lo, hi, layout, scale, use_mc, cfg)
-            step_ops = (op, moments)
-        elif clip:
-            # phase A in the bucket program (reduce-scatter into the fp32 shard + per-CTA Σx²); the update op runs in step()
-            st = opt._clip if getattr(opt, "_clip", None) is not None else self._clip_state(eng, bagua_ddp, bucket, flat.device)
-            shard = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
-            bucket._clip_shard = shard
-            row = st["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
+        rec = {"bucket": bucket.name, "group": self.process_group, "numel": flat.numel(), "lo": lo, "hi": hi, "layout": layout,
+               "state": (master, momentum, second) if is_adam or is_lamb else (master, momentum), "weights": wflat,
+               "param_ids": [id(t) for t in bucket.tensors], "shard": None}
+        bk.device = flat.device
+        if clip or is_lamb:
+            # phase A in the bucket program: reduce-scatter into the fp32 shard + per-CTA Σx² into this bucket's row of partials
+            # (read by the norm exchange; nothing reads them without clipping); the update runs in step()
+            if is_lamb and bk.lamb is None:
+                bk.lamb = self._lamb_state(eng, bagua_ddp, bucket, flat.device)
+            if clip and bk.clip is None:
+                bk.clip = self._clip_state(eng, bagua_ddp, bucket, flat.device)
+            row = (bk.clip if clip else bk.lamb)["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
+            shard = rec["shard"] = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
             red = C.ShardGradOp(eng.comm, bucket._slice.buf, bucket._slice.offset, nbytes, code, shard.data_ptr(), row.data_ptr(), scale, True, use_mc, cfg)
             bucket.backend_bucket.append_op(red)
             bucket._ops_keepalive.append(red)
-            coef_ptr = st["out"][1:].data_ptr()
-            if is_adam:
-                op = C.ShardAdamOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
-                                   second.data_ptr(), use_mc, cfg)
-            else:
-                op = C.ShardSgdOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
-                                  use_mc, cfg)
+            coef_ptr = bk.clip["out"][1:].data_ptr() if clip else 0
+        if is_lamb:
+            op, moments = self._lamb_ops(eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr)
+        elif clip and is_adam:
+            op = C.ShardAdamOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
+                               second.data_ptr(), use_mc, cfg)
+        elif clip:
+            op = C.ShardSgdOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
+                              use_mc, cfg)
         elif is_adam:
             op = C.AllReduceAdamOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                    master.data_ptr(), momentum.data_ptr(), second.data_ptr(), scale, True, use_mc, cfg)
         else:
             op = C.AllReduceSgdOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                   master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
-        if not (clip or is_lamb):
+        if clip or is_lamb:
+            bk.update_ops.append(op)
+        else:
             bucket.backend_bucket.append_op(op)
         bucket._ops_keepalive.append(op)
         kind = "fused_lamb_" if is_lamb else ("fused_adam_" if is_adam else "fused_sgd_")
         bucket.allreduce_variant = kind + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
-        opt._comm_ops.append(op)
-        if not hasattr(opt, "_comm_groups"):
-            opt._comm_groups = []
-        opt._comm_groups.append(group_index)
-        rec = {"bucket": bucket.name, "group": self.process_group, "numel": flat.numel(), "lo": lo, "hi": hi, "layout": layout,
-               "state": bucket._fused_state, "op": op, "weights": wflat, "param_ids": [id(t) for t in bucket.tensors]}
-        if step_ops is not None:
-            rec["step_ops"] = step_ops
+        rec["step_ops"] = (op, moments) if is_lamb else (op,)   # the update op first: state_dict() saves its count
+        bk.hyper_ops += [(o, group_index) for o in rec["step_ops"]]
+        bk.launches += len(rec["step_ops"])
         opt._register_shard(rec)
         opt._sync_hyper()
 
@@ -625,42 +597,27 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         names = [t.bagua_tensor_name for b in bagua_ddp.bagua_buckets for t in b.tensors if not t.bagua_tensor_name.startswith("bagua_padding_tensor")]
         box = eng.alloc(C.LambRatioOp.box_bytes(len(names)))
         bucket._companion_slices.append(box)
-        lam = {"index": {n: i for i, n in enumerate(names)}, "pending": set(names), "box": box,
-               "ratio": torch.ones(len(names), dtype=torch.float32, device=device),
-               "sums": torch.zeros(len(names), 2, dtype=torch.float64, device=device),
-               "seg_ptr": [0] * len(names), "seg_nblk": [0] * len(names), "ratio_op": None,
-               "partials": torch.zeros(len(bagua_ddp.bagua_buckets), C.MAX_COMM_BLOCKS, dtype=torch.float64, device=device)}
-        self.optimizer._lamb = lam
-        return lam
+        return {"index": {n: i for i, n in enumerate(names)}, "pending": set(names), "box": box,
+                "ratio": torch.ones(len(names), dtype=torch.float32, device=device),
+                "sums": torch.zeros(len(names), 2, dtype=torch.float64, device=device),
+                "seg_ptr": [0] * len(names), "seg_nblk": [0] * len(names), "ratio_op": None,
+                "partials": torch.zeros(len(bagua_ddp.bagua_buckets), C.MAX_COMM_BLOCKS, dtype=torch.float64, device=device)}
 
-    def _lamb_ops(self, eng, bagua_ddp, bucket, wslice, nbytes, code, lo, hi, layout, scale, use_mc, cfg):
-        """One bucket of the in-bucket LAMB: phase A (ShardGradOp) in the bucket program; the moments op over the shard's segments
-        (parameter ∩ [lo, hi), shard-local offsets), whose per-block partials the ratio exchange sums per parameter; the apply op.
-        The ratio exchange is built once every bucketed parameter has its table entry."""
+    def _lamb_ops(self, eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr):
+        """The LAMB ops of one bucket, after phase A: the moments op over the shard's segments (parameter ∩ [lo, hi), shard-local
+        offsets), whose per-block partials the ratio exchange sums per parameter, and the apply op. The ratio exchange is built once
+        every bucketed parameter has its table entry."""
         import torch
 
         from ...core import native
         from ...ops.optim import multi_tensor_plan
 
         C = native()
-        opt = self.optimizer
-        master, m1, m2 = bucket._fused_state
-        dev = master.device
-        lam = opt._lamb if opt._lamb is not None else self._lamb_state(eng, bagua_ddp, bucket, dev)
-        row_index = [b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)
-        shard = torch.zeros_like(master)
-        bucket._clip_shard = shard
-        coef_ptr = 0
-        if opt.max_grad_norm is not None:
-            st = opt._clip if getattr(opt, "_clip", None) is not None else self._clip_state(eng, bagua_ddp, bucket, dev)
-            row = st["partials"][row_index]
-            coef_ptr = st["out"][1:].data_ptr()
-        else:
-            row = lam["partials"][row_index]   # phase A writes its Σx² partials somewhere; nothing reads them without clipping
-        red = C.ShardGradOp(eng.comm, bucket._slice.buf, bucket._slice.offset, nbytes, code, shard.data_ptr(), row.data_ptr(), scale, True, use_mc, cfg)
-        bucket.backend_bucket.append_op(red)
+        lam = bk.lamb
+        master, m1, m2 = rec["state"]
+        shard, lo, hi, dev = rec["shard"], rec["lo"], rec["hi"], bk.device
         segs, views = [], [[], [], [], []]
-        for name, off, n, _, _ in layout:
+        for name, off, n, _, _ in rec["layout"]:
             a, b = max(off, lo), min(off + n, hi)
             if a < b:
                 segs.append((a - lo, b - lo, lam["index"][name]))
@@ -682,16 +639,16 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         table = torch.tensor([v for s in segs for v in s] or [0, 0, 0], dtype=torch.int32, device=dev)
         op = C.ShardLambOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, master.data_ptr(), m1.data_ptr(), m2.data_ptr(), table.data_ptr(), len(segs),
                            lam["ratio"].data_ptr(), use_mc, cfg)
-        bucket._ops_keepalive += [red, moments]
-        bucket._lamb_tables = (plan, partials, table, segs)
-        opt._lamb_moments.append(moments)
-        lam["pending"] -= {name for name, *_ in layout}
+        rec["lamb_tables"] = (plan, partials, table, segs)
+        bk.pre_ops.append(moments)
+        lam["pending"] -= {name for name, *_ in rec["layout"]}
         if not lam["pending"]:
             ptrs = torch.tensor(lam["seg_ptr"], dtype=torch.int64, device=dev)
             nblk = torch.tensor(lam["seg_nblk"], dtype=torch.int32, device=dev)
             lam["tables"] = (ptrs, nblk)
             lam["ratio_op"] = C.LambRatioOp(eng.comm, lam["box"].buf, lam["box"].offset, ptrs.data_ptr(), nblk.data_ptr(), len(lam["index"]),
                                             lam["ratio"].data_ptr(), lam["sums"].data_ptr())
+            bk.launches += 1
         return op, moments
 
 

@@ -56,12 +56,9 @@ class GraphedTrainStep:
                  optimizers: Sequence[torch.optim.Optimizer] = (), warmup: int = 3):
         self.model, self.train_step, self.optimizers = model, train_step, list(optimizers)
         for opt in self.optimizers:
-            if getattr(opt, "_comm_ops", None) is not None and getattr(opt, "max_grad_norm", None) is not None:
-                raise NotImplementedError("a sharded fused optimizer with max_grad_norm runs its norm exchange and clipped update from "
-                                          "step() with per-call host state (box parity, step count); it cannot be captured in a CUDA graph")
-            if getattr(opt, "_comm_ops", None) is not None and getattr(opt, "_kind", None) == "lamb":
-                raise NotImplementedError("the sharded fused LAMB optimizer runs its moments, ratio exchange and update from step() with "
-                                          "per-call host state (box parity, step count); it cannot be captured in a CUDA graph")
+            if getattr(opt, "native_ops_in_step", False):
+                raise NotImplementedError(f"{type(opt).__name__} runs native kernels from step() with per-call host state (box parity, "
+                                          "step count); it cannot be captured in a CUDA graph")
             why = graph_safe_optimizer(opt)
             if why is not None:
                 raise ValueError(f"optimizer cannot be captured in a CUDA graph: {why}")

@@ -400,7 +400,7 @@ def test_in_bucket_optimizers_also_update_parameters_outside_the_buckets():
         ref = torch.nn.Parameter(expert.detach().clone())
         opt = make([bucketed, expert], **kw)
         ropt = ref_cls([ref], **kw)
-        opt._comm_ops, opt._covered = [Op()], {id(bucketed)}     # what FusedGradientAllReduceAlgorithm sets up on a GPU box
+        opt._bucketing.hyper_ops, opt._bucketing.covered = [(Op(), 0)], {id(bucketed)}     # what FusedGradientAllReduceAlgorithm sets up on a GPU box
         before = bucketed.detach().clone()
         for _ in range(3):
             g = torch.randn(3, 4)
@@ -412,7 +412,7 @@ def test_in_bucket_optimizers_also_update_parameters_outside_the_buckets():
         torch.testing.assert_close(expert.detach(), ref.detach(), rtol=1e-5, atol=1e-6)
         assert torch.equal(bucketed.detach(), before)
         # the expert's optimizer state is part of the (otherwise shard-derived) checkpoint
-        opt._shards = [{"state": (), "group": None, "numel": 0, "layout": [], "lo": 0, "hi": 0, "op": Op(), "weights": None}]
+        opt._bucketing.shards = [{"state": (), "group": None, "numel": 0, "layout": [], "lo": 0, "hi": 0, "step_ops": (Op(),), "weights": None}]
         sd = opt.state_dict()
         assert sd["sharded_fused"] and len(sd["uncovered"]["state"]) == 1
         opt2 = make([torch.nn.Parameter(bucketed.detach().clone()), torch.nn.Parameter(expert.detach().clone())], **kw)
@@ -557,10 +557,11 @@ def _fused_init_operations_worker(rank, world):
                 assert isinstance(bucket.backend_bucket.ops[0], op_cls) and bucket.allreduce_variant.endswith("two_shot")
         finally:
             core.native = core_native
-        assert len(opt._comm_ops) == len(model.bagua_buckets) == len(opt._shards) and opt.collective_state_dict
-        assert all(op.hyper is not None for op in opt._comm_ops)
+        bk = opt._bucketing
+        assert len(bk.hyper_ops) == len(model.bagua_buckets) == len(bk.shards) and opt.collective_state_dict
+        assert all(op.hyper is not None for op, _ in bk.hyper_ops)
         if op_cls is AdamOp:   # every bucket op follows the weight decay of ITS parameter group
-            decays = {opt._comm_groups[i]: op.hyper[4] for i, op in enumerate(opt._comm_ops)}
+            decays = {group_index: op.hyper[4] for op, group_index in bk.hyper_ops}
             assert decays == {0: 0.1, 1: 0.0}, decays
         for n, p in model.named_parameters():   # weights now live in the "symmetric" slices, values and memory format unchanged
             assert torch.equal(p.detach(), want[n]) and p.stride() == want[n].stride()
@@ -570,7 +571,7 @@ def _fused_init_operations_worker(rank, world):
         for n in want:
             torch.testing.assert_close(sd["state"][n]["master"], want[n].contiguous())
             assert all(sd["state"][n][k].shape == want[n].shape for k in keys)
-        for rec in opt._shards:                  # perturb, restore, compare
+        for rec in bk.shards:                  # perturb, restore, compare
             for t in rec["state"]:
                 t.add_(1.0)
         opt.load_state_dict(sd)

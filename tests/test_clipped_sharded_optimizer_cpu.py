@@ -111,7 +111,7 @@ def _host_double_worker(rank, world):
             self.max_norm = m
 
         def run(self, opt):
-            clip = opt._clip
+            clip = opt._bucketing.clip
             assert clip["out"].data_ptr() == self.out_ptr and clip["extra"].data_ptr() == self.extra_ptr
             events.append(("norm", self.max_norm, float(clip["extra"])))
             clip["out"].copy_(torch.tensor([7.0, self.COEF]))
@@ -130,7 +130,7 @@ def _host_double_worker(rank, world):
             self.s = s
 
         def run(self, opt):
-            events.append(("update", opt._comm_ops.index(self)))
+            events.append(("update", opt._bucketing.update_ops.index(self)))
             self.s += 1
 
     class BackendBucket:
@@ -188,14 +188,15 @@ def _host_double_worker(rank, world):
             # phase A is the whole bucket program; the update ops are the optimizer's, one per bucket in bucket order
             assert all(len(b.backend_bucket.ops) == 1 and isinstance(b.backend_bucket.ops[0], GradDouble) for b in buckets)
             assert all("_clip_" in b.allreduce_variant for b in buckets)
-            assert len(opt._comm_ops) == len(buckets) and all(isinstance(op, UpdateOp) and op.hyper is not None for op in opt._comm_ops)
-            partials = opt._clip["partials"]
+            bk = opt._bucketing
+            assert len(bk.update_ops) == len(buckets) and all(isinstance(op, UpdateOp) and op.hyper is not None for op in bk.update_ops)
+            partials = bk.clip["partials"]
             assert partials.shape == (len(buckets), FakeC.MAX_COMM_BLOCKS) and partials.dtype == torch.float64
             for i, b in enumerate(buckets):
                 assert b.backend_bucket.ops[0].args[6] == partials[i].data_ptr()        # its own row of partial sums
-                assert b.backend_bucket.ops[0].args[5] == b._clip_shard.data_ptr()     # the shard phase B reads
-                assert opt._comm_ops[i].args[5] == b._clip_shard.data_ptr()
-                assert opt._comm_ops[i].args[6] == opt._clip["out"][1:].data_ptr()     # coef
+                assert b.backend_bucket.ops[0].args[5] == bk.shards[i]["shard"].data_ptr()     # the shard phase B reads
+                assert bk.update_ops[i].args[5] == bk.shards[i]["shard"].data_ptr()
+                assert bk.update_ops[i].args[6] == bk.clip["out"][1:].data_ptr()     # coef
             for n, p in model.named_parameters():
                 assert torch.equal(p.detach(), want[n])
 
@@ -240,10 +241,10 @@ def _host_double_worker(rank, world):
             assert sd["steps"] == 3 and set(want) <= set(sd["state"])
             for n in want:
                 assert all(sd["state"][n][k].shape == want[n].shape for k in keys)
-            for rec in opt._shards:
+            for rec in bk.shards:
                 for t in rec["state"]:
                     t.add_(1.0)
-                rec["op"].set_steps(0)
+                rec["step_ops"][0].set_steps(0)
             opt.load_state_dict(sd)
             again = opt.state_dict()
             assert again["steps"] == 3
@@ -253,7 +254,7 @@ def _host_double_worker(rank, world):
 
         # no bound configured, bucket ops live: clip_grad_norm_ would read consumed gradients -> refuse
         model, opt, _ = build(lambda ps, e: make_sharded_fused_sgd(ps, lr=0.1), extra)
-        assert opt._clip is None and all(not isinstance(b.backend_bucket.ops[0], GradDouble) for b in model.bagua_buckets)
+        assert opt._bucketing.clip is None and all(not isinstance(b.backend_bucket.ops[0], GradDouble) for b in model.bagua_buckets)
         with pytest.raises(RuntimeError, match="max_grad_norm"):
             opt.clip_grad_norm_(1.0)
         with pytest.raises(ValueError):

@@ -104,7 +104,7 @@ def _host_double_worker(rank, world):
 
     class Moments(Op):
         def run(self, opt):
-            events.append(("moments", opt._lamb_moments.index(self)))
+            events.append(("moments", opt._bucketing.pre_ops.index(self)))
             self.s += 1
 
     class Ratio(Op):
@@ -117,13 +117,13 @@ def _host_double_worker(rank, world):
 
     class Apply(Op):
         def run(self, opt):
-            events.append(("apply", opt._comm_ops.index(self)))
+            events.append(("apply", opt._bucketing.update_ops.index(self)))
             self.s += 1
 
     class Norm(Op):
         def run(self, opt):
             events.append(("norm",))
-            opt._clip["out"].copy_(torch.tensor([7.0, 0.5]))
+            opt._bucketing.clip["out"].copy_(torch.tensor([7.0, 0.5]))
 
     class BackendBucket:
         def __init__(self):
@@ -205,9 +205,9 @@ def _host_double_worker(rank, world):
                 model, opt, _ = build(lambda m: make_sharded_fused_lamb([{"params": list(m.parameters()), "weight_decay": 0.01}], lr=0.01),
                                       P=P, r=r, model=Odd())
                 (bucket,) = model.bagua_buckets
-                plan, partials, table, segs = bucket._lamb_tables
-                rec = opt._shards[0]
-                lam = opt._lamb
+                rec = opt._bucketing.shards[0]
+                plan, partials, table, segs = rec["lamb_tables"]
+                lam = opt._bucketing.lamb
                 layout = {name: (off, n) for name, off, n, _, _ in rec["layout"]}
                 for a, b, t in segs:
                     seen.setdefault(t, []).append((rec["lo"] + a, rec["lo"] + b))
@@ -219,7 +219,7 @@ def _host_double_worker(rank, world):
                     empty += 1
                     assert plan is None     # an empty slice still builds its ops (and takes part in every exchange)
                 assert lam["ratio_op"] is not None and len(lam["index"]) == 6   # the padding tensor has no ratio slot
-                assert opt._comm_ops[0].args[9] == len(segs)
+                assert opt._bucketing.update_ops[0].args[9] == len(segs)
             assert empty == (1 if P == 8 else 0)
             for t, spans in seen.items():   # every element of every parameter in exactly one segment, across the ranks
                 name = next(k for k, v in lam["index"].items() if v == t)
@@ -230,9 +230,9 @@ def _host_double_worker(rank, world):
 
         # a parameter longer than two 65536-element chunks: its segment gets consecutive stage-1 blocks, all summed for its ratio
         model, opt, _ = build(lambda m: make_sharded_fused_lamb(list(m.parameters()), lr=0.01), model=torch.nn.Linear(300, 500))
-        lam = opt._lamb
+        lam = opt._bucketing.lamb
         (bucket,) = model.bagua_buckets
-        plan, partials, table, segs = bucket._lamb_tables
+        plan, partials, table, segs = opt._bucketing.shards[0]["lamb_tables"]
         t_w = next(v for k, v in lam["index"].items() if k.endswith("weight"))
         t_b = next(v for k, v in lam["index"].items() if k.endswith("bias"))
         assert lam["seg_nblk"][t_w] == 3 and lam["seg_nblk"][t_b] == 1 and plan.n_blocks == 4
@@ -246,9 +246,10 @@ def _host_double_worker(rank, world):
             buckets = model.bagua_buckets
             assert all(len(b.backend_bucket.ops) == 1 for b in buckets), "phase A is the whole bucket program"
             assert all(b.allreduce_variant.startswith("fused_lamb_" + ("clip_" if bound else "")) for b in buckets)
-            assert len(opt._comm_ops) == len(opt._lamb_moments) == len(buckets)
-            coef_ptr = opt._clip["out"][1:].data_ptr() if bound else 0
-            assert all(m.args[7] == coef_ptr for m in opt._lamb_moments)
+            bk = opt._bucketing
+            assert len(bk.update_ops) == len(bk.pre_ops) == len(buckets)
+            coef_ptr = bk.clip["out"][1:].data_ptr() if bound else 0
+            assert all(m.args[7] == coef_ptr for m in bk.pre_ops)
             for n, p in model.named_parameters():
                 assert torch.equal(p.detach(), want[n])
             events.clear()
@@ -261,13 +262,13 @@ def _host_double_worker(rank, world):
             opt._gather = lambda t, group: [t]
             sd = opt.state_dict()
             assert sd["sharded_fused"] == "lamb" and sd["steps"] == 1 and set(want) <= set(sd["state"])
-            for rec in opt._shards:
+            for rec in bk.shards:
                 for t in rec["state"]:
                     t.add_(1.0)
                 for op in rec["step_ops"]:
                     op.set_steps(0)
             opt.load_state_dict(sd)
-            assert all(op.steps() == 1 for rec in opt._shards for op in rec["step_ops"])
+            assert all(op.steps() == 1 for rec in bk.shards for op in rec["step_ops"])
             again = opt.state_dict()
             for n in want:
                 for k in ("master", "exp_avg", "exp_avg_sq"):
@@ -280,7 +281,7 @@ def _host_double_worker(rank, world):
 
             # load_state_dict before with_bagua: applied to the shards when the ops are built
             model2, opt2, _ = build(lamb(bound), state=sd)
-            assert all(op.steps() == 1 for rec in opt2._shards for op in rec["step_ops"])
+            assert all(op.steps() == 1 for rec in opt2._bucketing.shards for op in rec["step_ops"])
             opt2._gather = lambda t, group: [t]
             for n in want:
                 assert torch.equal(opt2.state_dict()["state"][n]["exp_avg"], sd["state"][n]["exp_avg"])

@@ -250,9 +250,9 @@ def test_sharded_fused_optimizer_state_is_world_size_independent():
                 lo, hi = r * length, min((r + 1) * length, numel)
                 state = tuple(torch.zeros(length) for _ in range(n_state))
                 recs[r].append({"bucket": str(bi), "group": None, "numel": numel, "lo": lo, "hi": max(lo, hi), "layout": layout, "state": state,
-                                "op": Op(), "weights": torch.zeros(numel)})
+                                "step_ops": (Op(),), "weights": torch.zeros(numel)})
         for r, opt in enumerate(ranks):
-            opt._comm_ops = [rec["op"] for rec in recs[r]]
+            opt._bucketing.hyper_ops = [(rec["step_ops"][0], 0) for rec in recs[r]]
             for rec in recs[r]:
                 opt._register_shard(rec)
             # all-gather double: the same record of every rank, in rank order
@@ -276,7 +276,7 @@ def test_sharded_fused_optimizer_state_is_world_size_independent():
             for rec in src_recs[r]:
                 for k, t in zip(keys, rec["state"]):
                     t.copy_(shard_of(truth[k], rec["layout"], rec["numel"], rec["lo"], rec["hi"], t.numel()))
-                rec["op"].set_steps(17)
+                rec["step_ops"][0].set_steps(17)
         sds = [o.state_dict() for o in src]
         assert src[0].collective_state_dict and sds[0]["steps"] == 17 and sds[0]["param_groups"][0]["lr"] == 0.1
         for n in params:
@@ -288,7 +288,7 @@ def test_sharded_fused_optimizer_state_is_world_size_independent():
             o.load_state_dict(sds[0])
             assert o.param_groups[0]["lr"] == 0.025
             for rec in dst_recs[r]:
-                assert rec["op"].steps() == 17
+                assert rec["step_ops"][0].steps() == 17
                 for k, t in zip(keys, rec["state"]):
                     assert torch.equal(t, shard_of(truth[k], rec["layout"], rec["numel"], rec["lo"], rec["hi"], t.numel()))
         again = dst[1].state_dict()
@@ -303,4 +303,4 @@ def test_sharded_fused_optimizer_state_is_world_size_independent():
         for rec in fresh[2]:
             late._register_shard(rec)
             for k, t in zip(keys, rec["state"]):
-                assert torch.equal(t, shard_of(truth[k], rec["layout"], rec["numel"], rec["lo"], rec["hi"], t.numel())) and rec["op"].steps() == 17
+                assert torch.equal(t, shard_of(truth[k], rec["layout"], rec["numel"], rec["lo"], rec["hi"], t.numel())) and rec["step_ops"][0].steps() == 17

@@ -134,9 +134,9 @@ def _fused_sgd_rebucket_worker(rank, world):
         assert all(b.allreduce_variant.startswith("fused_sgd") for b in model.bagua_buckets)
         for it in range(8):
             if it == 4:
-                n_before = len(opt._shards)
+                n_before = len(opt._bucketing.shards)
                 model.bagua_ddp._reset_buckets()           # re-bucket mid-training
-                assert len(opt._shards) == n_before and len(opt._comm_ops) == n_before, "old shards must be dropped, not accumulated"
+                assert len(opt._bucketing.shards) == n_before and len(opt._bucketing.hyper_ops) == n_before, "old shards must be dropped, not accumulated"
                 assert opt._pending_state is None
             x = torch.randn(32, 512, device=dev, generator=torch.Generator(device=dev).manual_seed(it))
             opt.zero_grad()
