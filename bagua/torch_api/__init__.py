@@ -49,6 +49,7 @@ _ALIASES = {
     "model_parallel.moe.utils": "bagua_b200.parallel.moe.utils",
     "moe": "bagua_b200.parallel.moe",
     "ops": "bagua_b200.ops",
+    "amp": "bagua_b200.amp",
 }
 for _k, _v in _ALIASES.items():
     _m = _importlib.import_module(_v)

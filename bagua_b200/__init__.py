@@ -59,6 +59,7 @@ from . import contrib  # noqa: F401
 from . import ops  # noqa: F401
 from . import checkpoint  # noqa: F401
 from .parallel import moe  # noqa: F401
+from . import amp  # noqa: F401
 
 
 def version() -> str:

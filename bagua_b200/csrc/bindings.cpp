@@ -47,7 +47,8 @@ AdamParams make_adam(float lr, float b1, float b2, float eps, float wd, int step
 // set_hyper(<the rule's hyper-parameters in Hyper's field order>), steps() and set_steps(n) of an optimizer op.
 template <class Op, class... Args>
 void def_stepped(py::class_<Op, CommOp, std::shared_ptr<Op>>& cls) {
-    cls.def("set_hyper", [](Op& op, Args... args) { op.set_hyper({args...}); }).def("steps", &Op::steps).def("set_steps", &Op::set_steps);
+    cls.def("set_hyper", [](Op& op, Args... args) { op.set_hyper({args...}); }).def("steps", &Op::steps).def("set_steps", &Op::set_steps)
+        .def("set_device_step", &Op::set_device_step, py::arg("vote_ptr"), py::arg("step_ptr"));
 }
 }  // namespace
 
@@ -258,6 +259,12 @@ PYBIND11_MODULE(_C, m) {
              py::arg("partials_ptr"), py::arg("nslots"), py::arg("extra_ptr"), py::arg("out_ptr"))
         .def("set_max_norm", &GradNormOp::set_max_norm)
         .def("calls", &GradNormOp::calls);
+    py::class_<LossScaleNormOp, CommOp, std::shared_ptr<LossScaleNormOp>>(m, "LossScaleNormOp")
+        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, uint64_t, int, uint64_t, uint64_t, uint64_t>(), py::arg("comm"), py::arg("box"),
+             py::arg("box_off"), py::arg("partials_ptr"), py::arg("nslots"), py::arg("extra_ptr"), py::arg("out_ptr"), py::arg("step_ptr"))
+        .def("set_max_norm", &LossScaleNormOp::set_max_norm)
+        .def("set_scale_ptr", &LossScaleNormOp::set_scale_ptr)
+        .def("calls", &LossScaleNormOp::calls);
     def_stepped<ShardSgdOp, float, float, float, float, bool>(
         py::class_<ShardSgdOp, CommOp, std::shared_ptr<ShardSgdOp>>(m, "ShardSgdOp")
             .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(), py::arg("comm"),

@@ -49,6 +49,12 @@ void dispatch_mc(bool use_multimem, F&& f) {
         f(std::false_type{});
 }
 
+// f(std::bool_constant<on>{}) for any other compile-time switch of a kernel.
+template <typename F>
+void dispatch_flag(bool on, F&& f) {
+    dispatch_mc(on, f);
+}
+
 inline void check_launch(const char* what) {
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) throw std::runtime_error(std::string("bagua: launch of ") + what + " failed: " + cudaGetErrorString(e));

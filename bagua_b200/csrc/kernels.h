@@ -46,9 +46,13 @@ struct LambParams {
     float bias_correction2;  // 1 - beta2^t
 };
 
-// 1 - beta^step of the in-bucket Adam and LAMB ops and of FusedLAMB: in double, rounded once.
+// 1 - beta^step of the in-bucket Adam and LAMB ops and of FusedLAMB: in double, rounded once. Also callable from device code: the
+// kernels that take the step count from device memory (loss scaling) build their bias corrections with it.
+#ifdef __CUDACC__
+__host__ __device__
+#endif
 inline float bias_correction(float beta, uint64_t step) {
-    return static_cast<float>(1.0 - std::pow(static_cast<double>(beta), static_cast<double>(step)));
+    return static_cast<float>(1.0 - pow(static_cast<double>(beta), static_cast<double>(step)));
 }
 
 inline AdamParams adam_params(float lr, float beta1, float beta2, float eps, float weight_decay, bool adamw, uint64_t step) {
@@ -85,22 +89,32 @@ void launch_shard_grad(const PeerCtx& ctx, const PeerBuf& grads, size_t g_off, s
                        bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream);
 void launch_grad_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots, const double* extra, float max_norm,
                       uint32_t parity, float* out, cudaStream_t stream);
+//
+// Loss scaling: loss_scale_norm is grad_norm with the loss scale *scale read from device memory. With S the sum over all ranks,
+// out = {total = sqrt(S)/scale, coef = (1/scale)·min(max_norm/(total + 1e-6), 1) (max_norm = +inf: no bound), found_inf = !isfinite(S)}
+// and *step += !found_inf, the optimizer's effective step count. The phase-B launchers take that counter as `step` (nullable = the
+// behaviour above): `coef` then addresses {coef, found_inf}; on found_inf the kernel goes straight to its closing barrier, otherwise
+// hp's bias corrections / first_step are rebuilt on the device from t = *step.
+void launch_loss_scale_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots, const double* extra,
+                            const float* scale, float max_norm, uint32_t parity, float* out, uint32_t* step, cudaStream_t stream);
 void launch_shard_sgd(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                      float* master, float* momentum, const SgdParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream);
+                      float* master, float* momentum, const SgdParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream,
+                      const uint32_t* step = nullptr);
 void launch_shard_adam(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
                        float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, bool use_multimem, int nblocks, int nthreads,
-                       cudaStream_t stream);
+                       cudaStream_t stream, const uint32_t* step = nullptr);
 // In-bucket LAMB. The moments of every shard run as launch_multi_tensor_lamb_stage1 over the shard's segments (one parameter ∩ the
 // owned slice each). lamb_ratio: parameter t's local {Σw², Σu²} is the fixed-order sum of the seg_nblk[t] stage-1 partials at
 // seg_ptr[t] (0 blocks: no segment on this rank); the per-rank pairs are exchanged through the symmetric `box`
 // (2 halves · kMaxPeers · nparams double2 at box_off, half = parity) and summed in rank order → ratio[t] (fp32, identical bits on
 // every rank) and sums[t]. shard_lamb: w ← w − lr·r·u on the owned slice, r = ratio[segs[3s+2]] for the elements
 // [segs[3s], segs[3s+1]) of the shard (1 elsewhere, and everywhere when weight_decay == 0), then the weights are all-gathered.
+// `vote` = {coef, found_inf} and `step` as for launch_shard_sgd (both null without loss scaling).
 void launch_lamb_ratio(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const uint64_t* seg_ptr, const int32_t* seg_nblk, int nparams,
                        uint32_t parity, float* ratio, double* sums, cudaStream_t stream);
 void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, float* master, const float* exp_avg,
                        const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, const LambParams& hp, bool use_multimem,
-                       int nblocks, int nthreads, cudaStream_t stream);
+                       int nblocks, int nthreads, cudaStream_t stream, const float* vote = nullptr, const uint32_t* step = nullptr);
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,
                          int nblocks, int nthreads, cudaStream_t stream);
 void launch_peer_barrier(const PeerCtx& ctx, cudaStream_t stream);
@@ -228,9 +242,10 @@ void launch_multi_tensor_sgd_mp(const TensorListDesc& d, int dtype, bool has_mom
 // LAMB in two launches, lists [param(T), grad(T), exp_avg(f32), exp_avg_sq(f32)(, master(f32) when mixed)]. Stage 1: the moments with
 // g = grad·*coef (coef nullable = 1), fp64 {Σw², Σu²} of each block in sums[2·block], gradient cleared when zero_grad. Stage 2: each
 // block sums its tensor's block partials in a fixed order, forms the trust ratio and applies w ← w − lr·r·u (u recomputed from the
-// new moments); mixed writes the fp32 master and the parameter rounded once.
+// new moments); mixed writes the fp32 master and the parameter rounded once. With `step` (device, nullable) coef addresses
+// {coef, found_inf}: on found_inf stage 1 touches nothing, otherwise it takes its bias corrections from t = *step.
 void launch_multi_tensor_lamb_stage1(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const float* coef, double* sums, bool zero_grad,
-                                     cudaStream_t stream);
+                                     cudaStream_t stream, const uint32_t* step = nullptr);
 void launch_multi_tensor_lamb_stage2(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const double* sums, cudaStream_t stream);
 // QAdam momentum pre-step (bagua/torch_api/algorithms/q_adam.py:193-221): m = beta1*m + (1-beta1)*g
 void launch_qadam_momentum(float* exp_avg, const void* grad, int grad_dtype, size_t numel, float beta1, cudaStream_t stream);

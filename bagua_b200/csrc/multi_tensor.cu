@@ -352,10 +352,18 @@ void launch_multi_tensor_adam(const TensorListDesc& d, int dtype, const AdamPara
 // Stage 1 leaves one fp64 {Σw², Σu²} pair per block (sums[2·block], no atomics); a block belongs to exactly one tensor, so stage 2
 // gets a tensor's norms by adding its blocks' pairs in block order. Stage 2 recomputes u from the new moments and the unchanged w with
 // the same lamb_direction, so no per-element buffer holds u between the launches.
-template <typename T, bool MIXED>
+// DEV_STEP (the in-bucket LAMB with loss scaling): coef addresses {coef, found_inf} and *step is the effective step count including
+// this step; a skipped step returns before any write (its stale sums are not used), a taken one builds its bias corrections from t.
+template <typename T, bool MIXED, bool DEV_STEP>
 __global__ void __launch_bounds__(kThreads)
-    multi_tensor_lamb_stage1_kernel(TensorListDesc d, LambParams hp, const float* coef, double* sums, int zero_grad) {
+    multi_tensor_lamb_stage1_kernel(TensorListDesc d, LambParams hp, const float* coef, double* sums, int zero_grad, const uint32_t* step) {
     __shared__ double s_w[kThreads / 32], s_u[kThreads / 32];
+    if constexpr (DEV_STEP) {
+        if (coef[1] != 0.f) return;
+        const uint32_t ts = *step;
+        hp.bias_correction1 = bias_correction(hp.beta1, ts);
+        hp.bias_correction2 = bias_correction(hp.beta2, ts);
+    }
     const int t = d.block_to_tensor[blockIdx.x];
     const size_t off = static_cast<size_t>(d.block_to_chunk[blockIdx.x]) * d.chunk;
     const size_t n = static_cast<size_t>(d.sizes[t]);
@@ -430,14 +438,17 @@ __global__ void __launch_bounds__(kThreads) multi_tensor_lamb_stage2_kernel(Tens
 }
 
 void launch_multi_tensor_lamb_stage1(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const float* coef, double* sums, bool zero_grad,
-                                     cudaStream_t stream) {
+                                     cudaStream_t stream, const uint32_t* step) {
     if (d.n_blocks <= 0) return;
+    if (step != nullptr && coef == nullptr) throw std::runtime_error("bagua: multi_tensor_lamb_stage1 with a device step needs {coef, found_inf}");
     dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
         using T = decltype(tag);
-        if (mixed)
-            multi_tensor_lamb_stage1_kernel<T, true><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, coef, sums, zero_grad ? 1 : 0);
-        else
-            multi_tensor_lamb_stage1_kernel<T, false><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, coef, sums, zero_grad ? 1 : 0);
+        dispatch_flag(mixed, [&](auto mx) {
+            dispatch_flag(step != nullptr, [&](auto dev) {
+                multi_tensor_lamb_stage1_kernel<T, decltype(mx)::value, decltype(dev)::value><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, coef, sums,
+                                                                                                                                 zero_grad ? 1 : 0, step);
+            });
+        });
     });
     check_launch("multi_tensor_lamb_stage1");
 }

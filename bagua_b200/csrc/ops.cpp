@@ -123,6 +123,7 @@ void AllReduceOneShotOp::run(Bucket&, StreamHandle stream, int) {
 
 void AllReduceSgdOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("allreduce_sgd");
+    if (dev_step()) throw std::runtime_error("bagua: allreduce_sgd updates during backward and cannot take a device-side step count");
     launch_allreduce_sgd(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_),
                          reinterpret_cast<float*>(momentum_), params(), scale_, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
     steps_++;
@@ -140,6 +141,7 @@ void AllGatherOp::run(Bucket&, StreamHandle stream, int) {
 
 void AllReduceAdamOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("allreduce_adam");
+    if (dev_step()) throw std::runtime_error("bagua: allreduce_adam updates during backward and cannot take a device-side step count");
     launch_allreduce_adam(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_),
                           reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), params(), scale_, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads,
                           S(stream));
@@ -159,23 +161,32 @@ void GradNormOp::run(Bucket&, StreamHandle stream, int) {
     calls_++;
 }
 
+void LossScaleNormOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("loss_scale_norm");
+    launch_loss_scale_norm(comm_->ctx(), box_.buf, box_off_, reinterpret_cast<const double*>(partials_), nslots_, reinterpret_cast<const double*>(extra_),
+                           reinterpret_cast<const float*>(scale_), max_norm_, static_cast<uint32_t>(calls_ & 1u), reinterpret_cast<float*>(out_),
+                           reinterpret_cast<uint32_t*>(step_), S(stream));
+    calls_++;
+}
+
 void ShardSgdOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("shard_sgd");
-    launch_shard_sgd(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), reinterpret_cast<const float*>(coef_),
-                     reinterpret_cast<float*>(master_), reinterpret_cast<float*>(momentum_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
+    launch_shard_sgd(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), coef_or_vote(coef_),
+                     reinterpret_cast<float*>(master_), reinterpret_cast<float*>(momentum_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream),
+                     dev_step());
     steps_++;
 }
 
 void ShardAdamOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("shard_adam");
-    launch_shard_adam(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), reinterpret_cast<const float*>(coef_),
+    launch_shard_adam(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), coef_or_vote(coef_),
                       reinterpret_cast<float*>(master_), reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads,
-                      S(stream));
+                      S(stream), dev_step());
     steps_++;
 }
 
 void LambMomentsOp::run(Bucket&, StreamHandle stream, int) {
-    launch_multi_tensor_lamb_stage1(desc_, F32, false, params(), reinterpret_cast<const float*>(coef_), reinterpret_cast<double*>(partials_), false, S(stream));
+    launch_multi_tensor_lamb_stage1(desc_, F32, false, params(), coef_or_vote(coef_), reinterpret_cast<double*>(partials_), false, S(stream), dev_step());
     steps_++;
 }
 
@@ -190,7 +201,7 @@ void ShardLambOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("shard_lamb");
     launch_shard_lamb(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_), reinterpret_cast<const float*>(m1_),
                       reinterpret_cast<const float*>(m2_), reinterpret_cast<const int32_t*>(segs_), nsegs_, reinterpret_cast<const float*>(ratio_), params(), use_mc_,
-                      cfg_.nblocks, cfg_.nthreads, S(stream));
+                      cfg_.nblocks, cfg_.nthreads, S(stream), vote(), dev_step());
     steps_++;
 }
 

@@ -138,7 +138,10 @@ inline AdamParams device_params(const AdamHyper& h, uint64_t steps) {
 inline LambParams device_params(const LambHyper& h, uint64_t steps) { return lamb_params(h.lr, h.beta1, h.beta2, h.eps, h.weight_decay, steps + 1); }
 
 // An optimizer op: hyper-parameters published from Python (the forward pre-hook may do so while the comm worker runs the op, hence
-// the lock) and the count of launches so far, which checkpoints save and restore.
+// the lock) and the count of launches so far, which checkpoints save and restore. With loss scaling a launch may be a skipped step,
+// so the count that matters lives on the device: set_device_step(vote, step) hands the op the {coef, found_inf} pair and the
+// effective step counter that LossScaleNormOp maintains; the kernel then takes its gradient coefficient from `vote`, obeys
+// found_inf and derives the step-dependent parameters from *step instead of from steps().
 template <class Hyper>
 class SteppedOp : public CommOp {
 public:
@@ -148,8 +151,15 @@ public:
     }
     uint64_t steps() const { return steps_; }
     void set_steps(uint64_t s) { steps_ = s; }
+    void set_device_step(uint64_t vote, uint64_t step) {
+        if ((vote == 0) != (step == 0)) throw std::invalid_argument("bagua: an optimizer op takes the vote and the step counter together");
+        vote_ = vote, dev_step_ = step;
+    }
 
 protected:
+    const float* coef_or_vote(uint64_t coef) const { return reinterpret_cast<const float*>(vote_ ? vote_ : coef); }
+    const float* vote() const { return reinterpret_cast<const float*>(vote_); }
+    const uint32_t* dev_step() const { return reinterpret_cast<const uint32_t*>(dev_step_); }
     auto params() {
         std::lock_guard<std::mutex> lk(mu_);
         return device_params(hp_, steps_);
@@ -157,6 +167,7 @@ protected:
     uint64_t steps_ = 0;
 
 private:
+    uint64_t vote_ = 0, dev_step_ = 0;
     Hyper hp_;
     std::mutex mu_;
 };
@@ -282,6 +293,32 @@ private:
     int nslots_;
     uint64_t extra_, out_;
     float max_norm_ = 1.f;
+    uint64_t calls_ = 0;
+};
+
+// The norm exchange of an optimizer with loss scaling (see loss_scale_norm_kernel): GradNormOp with the loss scale read from device
+// memory at `scale` (settable: the scaler's tensor, or a constant 1), out = {total, coef, found_inf} and the effective step count
+// `step` (uint32, device) advanced on every step that is not skipped. max_norm = +inf: no clipping.
+class LossScaleNormOp final : public CommOp {
+public:
+    LossScaleNormOp(std::shared_ptr<PeerComm> comm, SymmBuf box, size_t box_off, uint64_t partials, int nslots, uint64_t extra, uint64_t out, uint64_t step)
+        : comm_(std::move(comm)), box_(box), box_off_(box_off), partials_(partials), nslots_(nslots), extra_(extra), out_(out), step_(step) {}
+    const char* kind() const override { return "loss_scale_norm"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return false; }  // the box half alternates with the call counter
+    void set_max_norm(float m) { max_norm_ = m; }
+    void set_scale_ptr(uint64_t scale) { scale_ = scale; }
+    uint64_t calls() const { return calls_; }
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf box_;
+    size_t box_off_;
+    uint64_t partials_;
+    int nslots_;
+    uint64_t extra_, out_, step_;
+    uint64_t scale_ = 0;
+    float max_norm_ = INFINITY;
     uint64_t calls_ = 0;
 };
 

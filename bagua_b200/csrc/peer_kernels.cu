@@ -422,10 +422,12 @@ __device__ __forceinline__ double ld_peer_f64(const void* p) {
 // call in between, so no closing barrier is needed. out = {total, coef}, coef = min(max_norm / (total + 1e-6), 1) in fp32 with
 // torch's operation order (reciprocal, then the product); a NaN norm gives a NaN coef, as in torch.
 constexpr int kNormThreads = 256;
-__global__ void __launch_bounds__(kNormThreads) grad_norm_kernel(PeerCtx ctx, PeerBuf box, size_t box_off, const double* partials, int nslots,
-                                                                 const double* extra, float max_norm, uint32_t parity, float* out) {
+
+// The exchange of both norm kernels: this rank's partials in a fixed order (+ *extra) → slot [rank] of every peer's box half →
+// barrier `epoch` → the P slots of the own box added in rank order into `sum` (thread 0 only). False when the barrier failed.
+__device__ __forceinline__ bool exchange_sumsq(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots,
+                                               const double* extra, uint32_t parity, uint32_t epoch, double& sum) {
     __shared__ double s_sum[kNormThreads];
-    const uint32_t e0 = load_epoch(ctx);
     double s = 0.0;
     for (int i = threadIdx.x; i < nslots; i += kNormThreads) s += partials[i];
     s_sum[threadIdx.x] = s;
@@ -440,19 +442,62 @@ __global__ void __launch_bounds__(kNormThreads) grad_norm_kernel(PeerCtx ctx, Pe
         const double mine = s_sum[0] + (extra != nullptr ? *extra : 0.0);
         st_peer_f64(box.ptr[threadIdx.x] + half + ctx.rank * sizeof(double), mine);
     }
-    const bool ok = peer_barrier(ctx, e0 + 1);
+    const bool ok = peer_barrier(ctx, epoch);
+    if (ok && threadIdx.x == 0) {
+        const char* mybox = box.ptr[ctx.rank] + half;
+        sum = 0.0;
+        for (int p = 0; p < ctx.world; ++p) sum += ld_peer_f64(mybox + p * sizeof(double));
+    }
+    return ok;
+}
+
+__global__ void __launch_bounds__(kNormThreads) grad_norm_kernel(PeerCtx ctx, PeerBuf box, size_t box_off, const double* partials, int nslots,
+                                                                 const double* extra, float max_norm, uint32_t parity, float* out) {
+    const uint32_t e0 = load_epoch(ctx);
+    double sum = 0.0;
+    const bool ok = exchange_sumsq(ctx, box, box_off, partials, nslots, extra, parity, e0 + 1, sum);
     if (threadIdx.x == 0) {
         float total = __int_as_float(0x7fc00000), coef = total;
         if (ok) {
-            const char* mybox = box.ptr[ctx.rank] + half;
-            double sum = 0.0;
-            for (int p = 0; p < ctx.world; ++p) sum += ld_peer_f64(mybox + p * sizeof(double));
             total = static_cast<float>(sqrt(sum));
             const float c = __fmul_rn(__frcp_rn(__fadd_rn(total, 1e-6f)), max_norm);
             coef = c > 1.f ? 1.f : c;
         }
         out[0] = total;
         out[1] = coef;
+    }
+    store_epoch(ctx, e0 + 1);
+}
+
+// The norm exchange of an optimizer with loss scaling: the same sum S, which is over the still-scaled gradient. Squares of finite
+// fp32 values cannot overflow an fp64 sum, so S is non-finite iff some reduced gradient element is: that is the overflow vote, and
+// every rank adds the same P numbers in the same order, so every rank casts the same one. out = {total, coef, found_inf} with
+// total = sqrt(S)/scale (the norm of the unscaled gradient), coef = float(1/scale)·clip, clip as in grad_norm_kernel on `total`
+// (1 when max_norm = +inf); *step, the optimizer's effective step count, advances unless the step is skipped. A failed barrier
+// votes "skip" and leaves the counter alone.
+__global__ void __launch_bounds__(kNormThreads) loss_scale_norm_kernel(PeerCtx ctx, PeerBuf box, size_t box_off, const double* partials, int nslots,
+                                                                       const double* extra, const float* scale, float max_norm, uint32_t parity,
+                                                                       float* out, uint32_t* step) {
+    const uint32_t e0 = load_epoch(ctx);
+    double sum = 0.0;
+    const bool ok = exchange_sumsq(ctx, box, box_off, partials, nslots, extra, parity, e0 + 1, sum);
+    if (threadIdx.x == 0) {
+        float total = __int_as_float(0x7fc00000), coef = total, found_inf = 1.f;
+        if (ok) {
+            const double inv = 1.0 / static_cast<double>(*scale);
+            total = static_cast<float>(sqrt(sum) * inv);
+            float clip = 1.f;
+            if (max_norm < INFINITY) {
+                const float c = __fmul_rn(__frcp_rn(__fadd_rn(total, 1e-6f)), max_norm);
+                clip = c > 1.f ? 1.f : c;
+            }
+            coef = __fmul_rn(static_cast<float>(inv), clip);
+            found_inf = isfinite(sum) ? 0.f : 1.f;
+            if (found_inf == 0.f) *step += 1u;
+        }
+        out[0] = total;
+        out[1] = coef;
+        out[2] = found_inf;
     }
     store_epoch(ctx, e0 + 1);
 }
@@ -479,26 +524,47 @@ __device__ __forceinline__ void update_owned_shard(const PeerCtx& ctx, const Pee
         });
 }
 
-template <typename T, int P, bool USE_MC>
+//
+// DEV_STEP (loss scaling): `coef` addresses {coef, found_inf} of loss_scale_norm_kernel and *step is the effective step count t that
+// includes this step. The vote has the same bits on every rank, so the branch on it is uniform across ranks and CTAs: a skipped step
+// touches no state, publishes nothing and only takes the closing barrier; a taken one rebuilds the step-dependent fields of hp from
+// t. Without DEV_STEP `step` is not read and hp is the host's.
+template <typename T, int P, bool USE_MC, bool DEV_STEP>
 __global__ void __launch_bounds__(512) shard_sgd_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
-                                                        const float* coef, float* master, float* momentum_buf, SgdParams hp) {
+                                                        const float* coef, float* master, float* momentum_buf, SgdParams hp, const uint32_t* step) {
     const uint32_t e0 = load_epoch(ctx);
     const float c = *coef;
-    update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard,
-                                     [&](size_t j, const float* g, float* w) { sgd_update<Vec16<T>::N>(master, momentum_buf, j, g, c, hp, w); });
+    bool skip = false;
+    if constexpr (DEV_STEP) {
+        skip = coef[1] != 0.f;
+        hp.first_step = *step == 1u ? 1 : 0;
+    }
+    if (!skip)
+        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard,
+                                         [&](size_t j, const float* g, float* w) { sgd_update<Vec16<T>::N>(master, momentum_buf, j, g, c, hp, w); });
     peer_barrier(ctx, e0 + 1);
     store_epoch(ctx, e0 + 1);
 }
 
-template <typename T, int P, bool USE_MC>
+template <typename T, int P, bool USE_MC, bool DEV_STEP>
 __global__ void __launch_bounds__(512) shard_adam_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
-                                                         const float* coef, float* master, float* exp_avg, float* exp_avg_sq, AdamParams hp) {
+                                                         const float* coef, float* master, float* exp_avg, float* exp_avg_sq, AdamParams hp,
+                                                         const uint32_t* step) {
     const uint32_t e0 = load_epoch(ctx);
     const float c = *coef;
-    const float inv_bc1 = 1.f / hp.bias_correction1, inv_sqrt_bc2 = rsqrtf(hp.bias_correction2);
-    update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard, [&](size_t j, const float* g, float* w) {
-        adam_update<Vec16<T>::N>(master, exp_avg, exp_avg_sq, j, g, c, hp, inv_bc1, inv_sqrt_bc2, w);
-    });
+    bool skip = false;
+    if constexpr (DEV_STEP) {
+        skip = coef[1] != 0.f;
+        const uint32_t t = *step;
+        hp.bias_correction1 = bias_correction(hp.beta1, t);
+        hp.bias_correction2 = bias_correction(hp.beta2, t);
+    }
+    if (!skip) {
+        const float inv_bc1 = 1.f / hp.bias_correction1, inv_sqrt_bc2 = rsqrtf(hp.bias_correction2);
+        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard, [&](size_t j, const float* g, float* w) {
+            adam_update<Vec16<T>::N>(master, exp_avg, exp_avg_sq, j, g, c, hp, inv_bc1, inv_sqrt_bc2, w);
+        });
+    }
     peer_barrier(ctx, e0 + 1);
     store_epoch(ctx, e0 + 1);
 }
@@ -560,13 +626,22 @@ __device__ __forceinline__ int lamb_segment_at(const int32_t* segs, int nsegs, i
 }
 
 // Apply and publish: w ← w − lr·r·u on the owned slice with u recomputed from the stage-1 moments (lamb_direction, the same code
-// that fed Σu²), all-gather of the weights, closing barrier — the walk of shard_adam_kernel over the fp32 master.
-template <typename T, int P, bool USE_MC>
+// that fed Σu²), all-gather of the weights, closing barrier — the walk of shard_adam_kernel over the fp32 master. DEV_STEP as for
+// shard_sgd_kernel, with vote = {coef, found_inf}: the bias corrections are the ones the moments kernel built from the same t.
+template <typename T, int P, bool USE_MC, bool DEV_STEP>
 __global__ void __launch_bounds__(512) shard_lamb_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, float* master, const float* exp_avg,
-                                                         const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, LambParams hp) {
+                                                         const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, LambParams hp,
+                                                         const float* vote, const uint32_t* step) {
     const uint32_t e0 = load_epoch(ctx);
     constexpr int N = Vec16<T>::N;
-    update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), master, [&](size_t j, const float* w0, float* w) {
+    bool skip = false;
+    if constexpr (DEV_STEP) {
+        skip = vote[1] != 0.f;
+        const uint32_t t = *step;
+        hp.bias_correction1 = bias_correction(hp.beta1, t);
+        hp.bias_correction2 = bias_correction(hp.beta2, t);
+    }
+    if (!skip) update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), master, [&](size_t j, const float* w0, float* w) {
         const float4* ap = reinterpret_cast<const float4*>(exp_avg + j * N);
         const float4* bp = reinterpret_cast<const float4*>(exp_avg_sq + j * N);
         int s = lamb_segment_at(segs, nsegs, static_cast<int64_t>(j * N));
@@ -911,15 +986,26 @@ void launch_grad_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, co
     check_launch("grad_norm");
 }
 
+void launch_loss_scale_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots, const double* extra,
+                            const float* scale, float max_norm, uint32_t parity, float* out, uint32_t* step, cudaStream_t stream) {
+    if (box_off % 8) throw std::runtime_error("bagua: loss_scale_norm box offset must be 8-byte aligned");
+    if (scale == nullptr || step == nullptr) throw std::runtime_error("bagua: loss_scale_norm needs the loss scale and the step counter");
+    loss_scale_norm_kernel<<<1, kNormThreads, 0, stream>>>(ctx, box, box_off, partials, nslots, extra, scale, max_norm, parity, out, step);
+    check_launch("loss_scale_norm");
+}
+
 void launch_shard_sgd(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                      float* master, float* momentum, const SgdParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream) {
+                      float* master, float* momentum, const SgdParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream,
+                      const uint32_t* step) {
     const size_t vecs = peer_vecs("shard_sgd", bytes, w_off, 0, nblocks);
     if (vecs == 0) return;
     dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
             dispatch_mc(use_multimem, [&](auto mc) {
-                shard_sgd_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
-                    ctx, weights, w_off, vecs, shard, coef, master, momentum, hp);
+                dispatch_flag(step != nullptr, [&](auto dev) {
+                    shard_sgd_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(dev)::value><<<nblocks, nthreads, 0, stream>>>(
+                        ctx, weights, w_off, vecs, shard, coef, master, momentum, hp, step);
+                });
             });
         });
     });
@@ -928,15 +1014,17 @@ void launch_shard_sgd(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, 
 
 void launch_shard_adam(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
                        float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, bool use_multimem, int nblocks, int nthreads,
-                       cudaStream_t stream) {
+                       cudaStream_t stream, const uint32_t* step) {
     const size_t vecs = peer_vecs("shard_adam", bytes, w_off, 0, nblocks);
     if (hp.amsgrad) throw std::runtime_error("bagua: shard_adam does not implement amsgrad");
     if (vecs == 0) return;
     dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
             dispatch_mc(use_multimem, [&](auto mc) {
-                shard_adam_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
-                    ctx, weights, w_off, vecs, shard, coef, master, exp_avg, exp_avg_sq, hp);
+                dispatch_flag(step != nullptr, [&](auto dev) {
+                    shard_adam_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(dev)::value><<<nblocks, nthreads, 0, stream>>>(
+                        ctx, weights, w_off, vecs, shard, coef, master, exp_avg, exp_avg_sq, hp, step);
+                });
             });
         });
     });
@@ -953,14 +1041,17 @@ void launch_lamb_ratio(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, c
 
 void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, float* master, const float* exp_avg,
                        const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, const LambParams& hp, bool use_multimem,
-                       int nblocks, int nthreads, cudaStream_t stream) {
+                       int nblocks, int nthreads, cudaStream_t stream, const float* vote, const uint32_t* step) {
     const size_t vecs = peer_vecs("shard_lamb", bytes, w_off, 0, nblocks);
+    if ((vote == nullptr) != (step == nullptr)) throw std::runtime_error("bagua: shard_lamb takes the vote and the step counter together");
     if (vecs == 0) return;
     dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
             dispatch_mc(use_multimem, [&](auto mc) {
-                shard_lamb_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
-                    ctx, weights, w_off, vecs, master, exp_avg, exp_avg_sq, segs, nsegs, ratio, hp);
+                dispatch_flag(step != nullptr, [&](auto dev) {
+                    shard_lamb_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(dev)::value><<<nblocks, nthreads, 0, stream>>>(
+                        ctx, weights, w_off, vecs, master, exp_avg, exp_avg_sq, segs, nsegs, ratio, hp, vote, step);
+                });
             });
         });
     });

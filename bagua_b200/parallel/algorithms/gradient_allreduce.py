@@ -96,7 +96,7 @@ class _Bucketing:
         self.hyper_ops = []    # (op, parameter-group index) of every op that takes hyper-parameters
         self.covered = set()   # ids of the bucketed parameters
         self.uncovered = None  # the parameters outside the buckets, looked up once
-        self.clip = None       # the norm exchange shared by all buckets (max_grad_norm), see _clip_state
+        self.clip = None       # the norm exchange shared by all buckets (max_grad_norm and / or loss_scaling), see _clip_state
         self.lamb = None       # the per-parameter ratio exchange shared by all buckets (LAMB), see _lamb_state
         # the program step() runs after the norm exchange, on the current stream of `device`: every bucket's pre-update op (LAMB
         # moments), LAMB's ratio exchange, every bucket's update op; empty when the updates run in the bucket kernels
@@ -115,6 +115,7 @@ class _ShardedStateMixin:
 
     _kind = "sgd"
     max_grad_norm = None
+    loss_scaling = False
 
     def __init__(self, *a, **k):
         super().__init__(*a, **k)
@@ -122,6 +123,7 @@ class _ShardedStateMixin:
         self._pending_state = None   # a checkpoint loaded while no shard exists, applied bucket by bucket by _register_shard
         self._norm_pending = False   # clip_grad_norm_ has computed this step's norm
         self._last_norm = None
+        self._loss_scale = None      # the device tensor the norm exchange reads the loss scale from (None: a constant 1)
 
     @property
     def collective_state_dict(self) -> bool:
@@ -130,9 +132,9 @@ class _ShardedStateMixin:
     @property
     def native_ops_in_step(self) -> bool:
         """Whether ``step()`` runs native kernels once the bucket kernels are live: the norm exchange and the clipped update with
-        ``max_grad_norm``, LAMB's moments, ratio exchange and update always. They carry per-call host state (box parity, step
-        count), so such a step cannot be captured in a CUDA graph."""
-        return self.max_grad_norm is not None or self._kind == "lamb"
+        ``max_grad_norm`` or ``loss_scaling``, LAMB's moments, ratio exchange and update always. They carry per-call host state
+        (box parity, step count), so such a step cannot be captured in a CUDA graph."""
+        return self.max_grad_norm is not None or self.loss_scaling or self._kind == "lamb"
 
     def _gather(self, t, group):
         import torch
@@ -152,6 +154,8 @@ class _ShardedStateMixin:
                 for name, full in consolidate_shards(self._gather(t, rec["group"]), rec["numel"], rec["layout"]).items():
                     state.setdefault(name, {})[key] = full.cpu()
             steps = max(steps, int(rec["step_ops"][0].steps()))
+        if self.loss_scaling:   # launches include skipped steps: the count that the kernels use is the device's
+            steps = int(self._bucketing.clip["t"].item())
         groups = [{k: v for k, v in g.items() if k != "params"} for g in self.param_groups]
         # parameters outside the buckets (MoE experts, ignored ones) are stepped by the base class: their state in torch's format
         return {"sharded_fused": self._kind, "steps": steps, "state": state, "param_groups": groups, "uncovered": super().state_dict()}
@@ -178,6 +182,8 @@ class _ShardedStateMixin:
             t.copy_(shard_of(per_name, rec["layout"], rec["numel"], rec["lo"], rec["hi"], t.numel(), device=t.device))
         for op in rec["step_ops"]:
             op.set_steps(int(sd.get("steps", 0)))
+        if self.loss_scaling:
+            self._bucketing.clip["t"].fill_(int(sd.get("steps", 0)))
 
     def refresh_master_weights(self):
         """Re-read the fp32 master shards from the model weights (call after loading or editing weights without optimizer
@@ -200,17 +206,20 @@ class _ShardedStateMixin:
             b.uncovered = [p for g in self.param_groups for p in g["params"] if id(p) not in b.covered]
         return [p for p in b.uncovered if p.grad is not None]
 
-    def _step_uncovered(self, coef=None):
+    def _step_uncovered(self, coef=None, found_inf=None):
         """Parameters that no bucket kernel updates — MoE experts (excluded from data parallelism), ignored parameters —
-        get the ordinary fused update here (their gradients scaled by the clipping coefficient ``coef`` first, when given);
-        their gradients are cleared like the bucketed ones."""
+        get the ordinary fused update here (their gradients scaled by the coefficient ``coef`` first, when given);
+        their gradients are cleared like the bucketed ones. Their kernels count steps on the host, so with loss scaling the vote
+        ``found_inf`` is read here — the one host synchronisation ``torch.amp.GradScaler.step`` also makes, and only for models
+        that have such parameters — and an overflowed step leaves them alone."""
         left = self._uncovered()
         if left:
             import torch
 
-            if coef is not None:
-                torch._foreach_mul_([p.grad for p in left], coef)
-            super().step(only={id(p) for p in left})
+            if found_inf is None or not bool(found_inf.item()):
+                if coef is not None:
+                    torch._foreach_mul_([p.grad for p in left], coef)
+                super().step(only={id(p) for p in left})
             torch._foreach_zero_([p.grad for p in left])
 
     # ---- global gradient-norm clipping (``max_grad_norm``) ---------------------------------------------------------------
@@ -219,6 +228,28 @@ class _ShardedStateMixin:
         """Global L2 norm of the averaged gradient at the last step that clipped: a device fp32 0-d tensor with the same bits on
         every rank, overwritten by the next step (no host synchronisation). ``None`` before the first one."""
         return self._last_norm
+
+    # ---- dynamic loss scaling (``loss_scaling``) --------------------------------------------------------------------------
+    @property
+    def last_step_skipped(self):
+        """Whether the last step overflowed and was skipped on every rank: a device fp32 0-d tensor (1.0 / 0.0, the same bits
+        on every rank), overwritten by the next step (no host synchronisation). ``None`` without ``loss_scaling`` or before the
+        bucket kernels are live."""
+        clip = self._bucketing.clip
+        return clip["out"][2] if self.loss_scaling and clip is not None else None
+
+    def set_loss_scale(self, scale):
+        """The loss scale of the following steps: a 1-element fp32 tensor on the optimizer's device that the norm exchange reads
+        when it runs (so a scaler may keep updating it in place), or ``None`` for a constant 1.
+        :class:`bagua_b200.amp.ShardedGradScaler` calls this from ``step()``."""
+        if not self.loss_scaling:
+            raise RuntimeError("this optimizer was built without loss_scaling=True")
+        if scale is not None and (scale.numel() != 1 or str(scale.dtype) != "torch.float32"):
+            raise ValueError("the loss scale must be a 1-element fp32 tensor")
+        if self._norm_pending and scale is not self._loss_scale:
+            raise RuntimeError("clip_grad_norm_() has already computed this step's norm with another loss scale; hand the scale to the "
+                               "optimizer before clipping (ShardedGradScaler.attach(optimizer)), or clip with max_grad_norm")
+        self._loss_scale = scale
 
     def clip_grad_norm_(self, max_norm: float, norm_type: float = 2.0):
         """Clip by the global L2 norm of the averaged gradient with bound ``max_norm`` for this step and return the norm (device
@@ -239,6 +270,9 @@ class _ShardedStateMixin:
             raise RuntimeError("the in-bucket optimizer applied this step's update during backward, so its gradients cannot be clipped "
                                "afterwards; construct it with max_grad_norm=... (make_sharded_fused_sgd / make_sharded_fused_adam) to clip "
                                "on this path")
+        if self.loss_scaling and self._norm_pending:
+            raise RuntimeError("with loss_scaling the norm exchange also casts the overflow vote and counts the step: clip_grad_norm_() can "
+                               "run once per step")
         return self._launch_norm(max_norm).clone()
 
     def _launch_norm(self, max_norm):
@@ -254,7 +288,13 @@ class _ShardedStateMixin:
         elif clip["extra_set"]:
             clip["extra"].zero_()
             clip["extra_set"] = False
-        clip["norm_op"].set_max_norm(float(max_norm))
+        if self.loss_scaling:   # the norm and the bound are the unscaled gradient's; no bound: the exchange only unscales and votes
+            scale = clip["unit"] if self._loss_scale is None else self._loss_scale
+            if scale.device != clip["out"].device:
+                raise ValueError(f"the loss scale lives on {scale.device}, the optimizer's buckets on {clip['out'].device}")
+            clip["scale"] = scale   # kept alive until the next exchange has replaced it
+            clip["norm_op"].set_scale_ptr(scale.data_ptr())
+        clip["norm_op"].set_max_norm(float("inf") if max_norm is None else float(max_norm))
         dev = clip["out"].device
         native().run_op(clip["norm_op"], torch.cuda.current_stream(dev).cuda_stream, dev.index)
         self.kernel_launches += 1
@@ -264,10 +304,15 @@ class _ShardedStateMixin:
 
     def step(self, closure=None):
         """Without a peer engine: the flat optimizer (clipping first with ``max_grad_norm``). Otherwise: publish the
-        hyper-parameters; with ``max_grad_norm`` run the norm exchange (unless ``clip_grad_norm_`` ran it); run the step program
-        of the bucketing on the current stream (see :class:`_Bucketing`; empty when the bucket kernels of this iteration's backward
-        already applied the update); then step the parameters outside the buckets, their gradients scaled by the clipping
-        coefficient. No host synchronisation."""
+        hyper-parameters; with ``max_grad_norm`` or ``loss_scaling`` run the norm exchange (unless ``clip_grad_norm_`` ran it);
+        run the step program of the bucketing on the current stream (see :class:`_Bucketing`; empty when the bucket kernels of
+        this iteration's backward already applied the update); then step the parameters outside the buckets, their gradients
+        scaled by the exchange's coefficient. No host synchronisation, except with ``loss_scaling`` when the model has parameters
+        outside the buckets (see ``_step_uncovered``).
+
+        With ``loss_scaling`` the exchange also unscales by the loss scale (``set_loss_scale``; 1 when ``step()`` is called
+        without a scaler) and votes on overflow: a step whose averaged gradient holds an inf or a NaN changes no weight, no
+        optimizer state and not the step count, on any rank (``last_step_skipped``)."""
         b = self._bucketing
         if not b.hyper_ops:
             if self.max_grad_norm is not None and not self._norm_pending:
@@ -275,12 +320,13 @@ class _ShardedStateMixin:
             self._norm_pending = False
             return super().step(closure)
         self._sync_hyper()
-        coef = None
+        coef = found_inf = None
         if b.clip is not None:
             if not self._norm_pending:
                 self._launch_norm(self.max_grad_norm)
             self._norm_pending = False
             coef = b.clip["out"][1]
+            found_inf = b.clip["out"][2] if self.loss_scaling else None
         if b.update_ops:
             # Ordering: the post-backward hook made this stream wait for the comm stream, so every phase-A bucket kernel (shard +
             # partials) has finished; the next iteration's bucket launches wait for ready events recorded after this step() on
@@ -299,7 +345,7 @@ class _ShardedStateMixin:
                 C.run_op(b.lamb["ratio_op"], stream, dev)
             for op in b.update_ops:
                 C.run_op(op, stream, dev)
-        self._step_uncovered(coef)
+        self._step_uncovered(coef, found_inf)
         self._grads_zeroed = True
         self.kernel_launches += b.launches
         return None
@@ -327,7 +373,7 @@ def _check_bound(max_grad_norm):
     return None if max_grad_norm is None else float(max_grad_norm)
 
 
-def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, max_grad_norm=None):
+def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, max_grad_norm=None, loss_scaling=False):
     """SGD whose update runs *inside* each bucket's NVSwitch kernel (``allreduce_sgd_kernel``): reduce-scatter of the
     gradients → SGD(momentum) on this rank's 1/N shard with fp32 master weights → all-gather of the updated weights, one
     launch per bucket, overlapped with the rest of backward.  Optimizer state is sharded N ways (ZeRO-1-like) and the
@@ -337,7 +383,12 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
     ``max_grad_norm``: clip by the global L2 norm of the averaged gradient, as ``torch.nn.utils.clip_grad_norm_`` after a
     data-parallel all-reduce.  The bucket kernels then only reduce-scatter the gradients into an fp32 shard during backward
     (4 bytes per element / N of extra memory) and ``step()`` runs the norm exchange and the clipped update; see
-    ``docs/algorithms.md``."""
+    ``docs/algorithms.md``.
+
+    ``loss_scaling``: dynamic loss scaling for fp16 training, driven by :class:`bagua_b200.amp.ShardedGradScaler`. The bucket
+    program is the one of ``max_grad_norm`` (which stays optional: the norm it bounds and reports is the unscaled gradient's);
+    the norm exchange also divides by the loss scale and decides, with the same bits on every rank, whether the step overflowed;
+    an overflowed step changes nothing anywhere and does not count (``last_step_skipped``)."""
     from ...ops.optim import FusedSGD
 
     class _ShardedFusedSGD(_ShardedStateMixin, FusedSGD, ShardedFusedSGD):
@@ -345,7 +396,7 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
 
     opt = _ShardedFusedSGD(params, lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
                            master_weights=True, zero_grad_in_step=True)
-    opt.max_grad_norm = _check_bound(max_grad_norm)
+    opt.max_grad_norm, opt.loss_scaling = _check_bound(max_grad_norm), bool(loss_scaling)
     return opt
 
 
@@ -353,11 +404,11 @@ class ShardedFusedAdam(object):
     """Marker mix-in: see :func:`make_sharded_fused_adam`."""
 
 
-def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False, max_grad_norm=None):
+def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False, max_grad_norm=None, loss_scaling=False):
     """Adam / AdamW counterpart of :func:`make_sharded_fused_sgd`: the update of this rank's 1/N shard (fp32 master weights
     and both moments) runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_adam_kernel``).  With one
-    process (or without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedAdam`.  ``max_grad_norm``: see
-    :func:`make_sharded_fused_sgd`."""
+    process (or without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedAdam`.  ``max_grad_norm``,
+    ``loss_scaling``: see :func:`make_sharded_fused_sgd`."""
     from ...ops.optim import FusedAdam
 
     class _ShardedFusedAdam(_ShardedStateMixin, FusedAdam, ShardedFusedAdam):
@@ -365,7 +416,7 @@ def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weigh
 
     opt = _ShardedFusedAdam(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, adamw=adamw, master_weights=True,
                             zero_grad_in_step=True)
-    opt.max_grad_norm = _check_bound(max_grad_norm)
+    opt.max_grad_norm, opt.loss_scaling = _check_bound(max_grad_norm), bool(loss_scaling)
     return opt
 
 
@@ -373,7 +424,7 @@ class ShardedFusedLamb(object):
     """Marker mix-in: see :func:`make_sharded_fused_lamb`."""
 
 
-def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01, max_grad_norm=None):
+def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01, max_grad_norm=None, loss_scaling=False):
     """LAMB (apex ``FusedLAMB`` semantics, see :class:`bagua_b200.ops.optim.FusedLAMB`) on the in-bucket sharded path: each rank
     keeps fp32 master weights and both moments for its 1/N slice of every bucket.
 
@@ -384,14 +435,15 @@ def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weigh
     exchange of the per-parameter sums between the ranks (every rank obtains the same fp32 ratios), and the update plus the
     all-gather of the weights per bucket — ``2·buckets + 1`` launches (+1 with clipping). A parameter group with
     ``weight_decay=0`` gets no layer adaptation (ratio 1). With one process, or without a peer engine, it behaves like
-    :class:`bagua_b200.ops.optim.FusedLAMB`; see ``docs/algorithms.md``."""
+    :class:`bagua_b200.ops.optim.FusedLAMB`; see ``docs/algorithms.md``. ``loss_scaling``: see :func:`make_sharded_fused_sgd`;
+    a skipped step also leaves the moments alone, and its ratio exchange runs with an unused result."""
     from ...ops.optim import FusedLAMB
 
     class _ShardedFusedLamb(_ShardedStateMixin, FusedLAMB, ShardedFusedLamb):
         _kind = "lamb"
 
     opt = _ShardedFusedLamb(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, master_weights=True, zero_grad_in_step=True)
-    opt.max_grad_norm = _check_bound(max_grad_norm)
+    opt.max_grad_norm, opt.loss_scaling = _check_bound(max_grad_norm), bool(loss_scaling)
     return opt
 
 
@@ -458,10 +510,12 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
                 buckets.append(bk)
         return buckets
 
-    def _clip_state(self, eng, bagua_ddp, bucket, device):
+    def _clip_state(self, eng, bagua_ddp, bucket, device, scaled):
         """Buffers of the norm exchange, shared by all buckets: fp64 partial sums [bucket][CTA] (slots of unused CTAs stay 0), the
         fp64 Σx² of the parameters outside the buckets, out = {total, coef} in fp32, and the symmetric norm box (2·MAX_PEERS doubles,
-        freed with the first bucket's other symmetric slices when the buckets are rebuilt)."""
+        freed with the first bucket's other symmetric slices when the buckets are rebuilt). With loss scaling (``scaled``) the
+        exchange is LossScaleNormOp: out = {total, coef, found_inf}, ``t`` is the effective step count it advances (32 bits on the
+        device) and ``unit`` the scale of a step taken without a scaler."""
         import torch
 
         from ...core import native
@@ -469,10 +523,15 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         C = native()
         st = {"partials": torch.zeros(len(bagua_ddp.bagua_buckets), C.MAX_COMM_BLOCKS, dtype=torch.float64, device=device),
               "extra": torch.zeros((), dtype=torch.float64, device=device), "extra_set": False,
-              "out": torch.zeros(2, dtype=torch.float32, device=device)}
+              "out": torch.zeros(3 if scaled else 2, dtype=torch.float32, device=device)}
         box = eng.alloc(2 * C.MAX_PEERS * 8)
         bucket._companion_slices.append(box)
         st["box"] = box
+        if scaled:
+            st["t"], st["unit"] = torch.zeros(1, dtype=torch.int32, device=device), torch.ones(1, dtype=torch.float32, device=device)
+            st["norm_op"] = C.LossScaleNormOp(eng.comm, box.buf, box.offset, st["partials"].data_ptr(), st["partials"].numel(), st["extra"].data_ptr(),
+                                              st["out"].data_ptr(), st["t"].data_ptr())
+            return st
         st["norm_op"] = C.GradNormOp(eng.comm, box.buf, box.offset, st["partials"].data_ptr(), st["partials"].numel(), st["extra"].data_ptr(),
                                      st["out"].data_ptr())
         return st
@@ -537,32 +596,33 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         scale = (1.0 / n) if self.average else 1.0
         code = dtype_code(flat.dtype)
         second = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device) if is_adam or is_lamb else None
-        clip = opt.max_grad_norm is not None
+        clip, scaled = opt.max_grad_norm is not None, opt.loss_scaling
+        exchange = clip or scaled   # the norm exchange runs in step(), so the update does too
         layout = [(t.bagua_tensor_name, (t.bagua_getter_closure().data_ptr() - base) // flat.element_size(), t.bagua_getter_closure().numel(),
                    tuple(t.shape), tuple(dense_strides(t))) for t in bucket.tensors if not t.bagua_tensor_name.startswith("bagua_padding_tensor")]
         rec = {"bucket": bucket.name, "group": self.process_group, "numel": flat.numel(), "lo": lo, "hi": hi, "layout": layout,
                "state": (master, momentum, second) if is_adam or is_lamb else (master, momentum), "weights": wflat,
                "param_ids": [id(t) for t in bucket.tensors], "shard": None}
         bk.device = flat.device
-        if clip or is_lamb:
+        if exchange or is_lamb:
             # phase A in the bucket program: reduce-scatter into the fp32 shard + per-CTA Σx² into this bucket's row of partials
             # (read by the norm exchange; nothing reads them without clipping); the update runs in step()
             if is_lamb and bk.lamb is None:
                 bk.lamb = self._lamb_state(eng, bagua_ddp, bucket, flat.device)
-            if clip and bk.clip is None:
-                bk.clip = self._clip_state(eng, bagua_ddp, bucket, flat.device)
-            row = (bk.clip if clip else bk.lamb)["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
+            if exchange and bk.clip is None:
+                bk.clip = self._clip_state(eng, bagua_ddp, bucket, flat.device, scaled)
+            row = (bk.clip if exchange else bk.lamb)["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
             shard = rec["shard"] = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
             red = C.ShardGradOp(eng.comm, bucket._slice.buf, bucket._slice.offset, nbytes, code, shard.data_ptr(), row.data_ptr(), scale, True, use_mc, cfg)
             bucket.backend_bucket.append_op(red)
             bucket._ops_keepalive.append(red)
-            coef_ptr = bk.clip["out"][1:].data_ptr() if clip else 0
+            coef_ptr = bk.clip["out"][1:].data_ptr() if exchange else 0
         if is_lamb:
             op, moments = self._lamb_ops(eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr)
-        elif clip and is_adam:
+        elif exchange and is_adam:
             op = C.ShardAdamOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
                                second.data_ptr(), use_mc, cfg)
-        elif clip:
+        elif exchange:
             op = C.ShardSgdOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
                               use_mc, cfg)
         elif is_adam:
@@ -571,14 +631,17 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         else:
             op = C.AllReduceSgdOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                   master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
-        if clip or is_lamb:
+        if exchange or is_lamb:
             bk.update_ops.append(op)
         else:
             bucket.backend_bucket.append_op(op)
         bucket._ops_keepalive.append(op)
         kind = "fused_lamb_" if is_lamb else ("fused_adam_" if is_adam else "fused_sgd_")
-        bucket.allreduce_variant = kind + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
+        bucket.allreduce_variant = kind + ("scaled_" if scaled else "") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
         rec["step_ops"] = (op, moments) if is_lamb else (op,)   # the update op first: state_dict() saves its count
+        if scaled:   # the ops obey the exchange's vote and take the step count it keeps on the device
+            for o in rec["step_ops"]:
+                o.set_device_step(coef_ptr, bk.clip["t"].data_ptr())
         bk.hyper_ops += [(o, group_index) for o in rec["step_ops"]]
         bk.launches += len(rec["step_ops"])
         opt._register_shard(rec)

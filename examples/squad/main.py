@@ -20,7 +20,9 @@ What each part is here (nothing is imported from ``transformers``; there is no n
 * optimisation — AdamW (decay on matrices only) with linear warm-up / decay, gradient clipping, gradient accumulation through
   ``model.bagua_ddp.require_backward_grad_sync`` (micro-steps accumulate locally, the last one communicates).  On GPUs parameters are
   bf16 with fp32 master weights inside ``bagua_b200.ops.FusedAdam`` (``--fp16`` is accepted and means this mixed-precision path;
-  ``--dtype fp32`` restores full precision); ``--fused-shard`` moves AdamW into the bucket kernels; ``--fuse-optimizer`` uses the
+  ``--dtype fp32`` restores full precision; ``--dtype fp16`` trains in real fp16 with dynamic loss scaling, which needs
+  ``--fused-shard``: ``ShardedGradScaler`` unscales, detects overflow and skips steps on the device); ``--fused-shard`` moves AdamW
+  into the bucket kernels; ``--fuse-optimizer`` uses the
   generic ``bagua.contrib.fuse_optimizer``; ``--load-balance`` batches by non-pad length (LoadBalancingDistributedSampler).
 * evaluation — every rank scores a shard of the dev features, rank 0 decodes and writes predictions.json / nbest_predictions.json
   (and null_odds-free v2 handling) to ``--output_dir``; ``--evaluate_during_training`` does so every ``--logging_steps``.
@@ -110,7 +112,7 @@ def parse():
     a("--fuse-optimizer", action="store_true")
     a("--fused-shard", action="store_true", help="AdamW inside the bucket kernels (reduce-scatter → update → all-gather)")
     a("--load-balance", action="store_true", help="LoadBalancingDistributedSampler keyed on the number of non-pad tokens")
-    a("--dtype", default="bf16", choices=["bf16", "fp32"])
+    a("--dtype", default="bf16", choices=["bf16", "fp32", "fp16"], help="fp16: real fp16 with dynamic loss scaling, needs --fused-shard")
     a("--tiny", action="store_true", help="2-layer model (smoke tests)")
     a("--num-synthetic", type=int, default=256, help="paragraphs of generated SQuAD-format data when no file is given")
     args = p.parse_args()
@@ -252,7 +254,8 @@ def make_optimizer(args, model, cuda, world):
         return opt, q_adam.QAdamAlgorithm(opt)
     if args.fused_shard and cuda and args.algorithm == "gradient_allreduce":
         opt = make_sharded_fused_adam(groups, lr=args.learning_rate, eps=args.adam_epsilon, adamw=True,   # buckets are cut per parameter group
-                                      max_grad_norm=args.max_grad_norm if args.max_grad_norm > 0 else None)   # clipped inside step()
+                                      max_grad_norm=args.max_grad_norm if args.max_grad_norm > 0 else None,   # clipped inside step()
+                                      loss_scaling=args.dtype == "fp16")
         return opt, FusedGradientAllReduceAlgorithm(opt)
     if cuda and not args.fuse_optimizer:
         opt = bagua.ops.FusedAdam(groups, lr=args.learning_rate, eps=args.adam_epsilon, adamw=True)
@@ -314,6 +317,9 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
 
     sharded = isinstance(optimizer, ShardedFusedAdam)
     grad_norm = None
+    # fp16: the scaler hands its device scale to the sharded optimizer, whose step program unscales, votes on overflow and skips
+    scaler = bagua.amp.ShardedGradScaler() if args.dtype == "fp16" else None
+    skipped = torch.zeros((), device=dev) if scaler is not None else None   # accumulated on the device, read when logging
     step, seen_iters, loss_sum, loss_n, t_log, done = 0, 0, 0.0, 0, time.time(), False
     last_loss = None
     for epoch in range(epochs):
@@ -331,7 +337,7 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
                 with nvtx("forward"):
                     loss = model(ids, token_type_ids=tt, attention_mask=am, start_positions=sp, end_positions=ep)[0] / accum
                 with nvtx("backward"):
-                    loss.backward()
+                    (loss if scaler is None else scaler.scale(loss)).backward()
                 seen_iters += 1
                 if not last_micro:
                     continue
@@ -340,7 +346,12 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
                         if args.algorithm in ("gradient_allreduce", "bytegrad"):
                             model.bagua_ddp.wait_pending_comm_ops()   # clip the COMMUNICATED gradient (the reference clips after backward, :262-267)
                         grad_norm = torch.nn.utils.clip_grad_norm_(model.parameters(), args.max_grad_norm)
-                    optimizer.fuse_step() if args.fuse_optimizer else optimizer.step()
+                    if scaler is not None:
+                        scaler.step(optimizer)
+                        skipped += optimizer.last_step_skipped
+                        scaler.update()
+                    else:
+                        optimizer.fuse_step() if args.fuse_optimizer else optimizer.step()
                     if sharded:   # the sharded optimizer clipped inside step() (max_grad_norm)
                         grad_norm = optimizer.last_grad_norm
                     scheduler.step()
@@ -351,7 +362,9 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
                 loss_sum, loss_n = loss_sum + last_loss.item(), loss_n + 1
                 rate = args.per_gpu_train_batch_size * accum * world * args.logging_steps / max(time.time() - t_log, 1e-9)
                 gn = "-" if grad_norm is None else f"{float(grad_norm):.4f}"
-                log.info("epoch %d step %d/%d loss %.4f lr %.3g grad norm %s %.1f samples/s", epoch, step, total, last_loss.item(), scheduler.get_last_lr()[0], gn, rate)
+                amp = "" if scaler is None else f" loss scale {scaler.get_scale():.0f} skipped {int(skipped.item())}"
+                log.info("epoch %d step %d/%d loss %.4f lr %.3g grad norm %s%s %.1f samples/s", epoch, step, total, last_loss.item(), scheduler.get_last_lr()[0], gn, amp,
+                         rate)
                 if args.evaluate_during_training:
                     res = evaluate(args, model, tokenizer, dev, rank, world, prefix=str(step))
                     log.info("  step %d: exact %.2f f1 %.2f", step, res["exact"], res["f1"])
@@ -396,7 +409,9 @@ def main():
         if getattr(args, flag):
             log.info("--%s is accepted for command-line compatibility and has no effect here", flag)
     dev = torch.device("cuda", bagua.get_local_rank()) if cuda else torch.device("cpu")
-    dtype = torch.bfloat16 if (cuda and args.dtype == "bf16") else torch.float32
+    if args.dtype == "fp16" and not (cuda and args.fused_shard and args.algorithm == "gradient_allreduce"):
+        raise SystemExit("--dtype fp16 needs a GPU, --fused-shard and --algorithm gradient_allreduce (loss scaling runs in the in-bucket optimizer)")
+    dtype = {"bf16": torch.bfloat16, "fp16": torch.float16}.get(args.dtype, torch.float32) if cuda else torch.float32
 
     model = build_model(args)
     tok_src = args.tokenizer_name or (args.model_name_or_path if os.path.isdir(args.model_name_or_path) else "")
