@@ -6,6 +6,12 @@
 //   fwd : y = relu(conv_out + bias)                       (in place)          | out, idx = maxpool2(relu(conv_out + bias))
 //   bwd : g' = g * (y > 0);  bias_grad += Σ g'                               | g_in = scatter(g * (out > 0), idx);  bias_grad += Σ
 // The convolution itself stays a library call (cuDNN); it is run without bias so cuDNN skips its own bias-grad reduction.
+//
+// NaN follows torch: relu(NaN) = NaN, its gradient passes (the mask is !(y <= 0), as in threshold_backward), and the pool's
+// argmax is the first maximum in scan order (0,0), (0,1), (1,0), (1,1) unless the window holds a NaN, then it is the last NaN
+// (max_pool2d's `val > max || isnan(val)`). The window max is taken over the pre-bias input (bias and ReLU are monotone).
+// Every pointer is accessed with 16-byte vectors (the pool's argmax bytes with 8-byte words); the launchers reject a
+// misaligned one before anything reaches the device.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -30,6 +36,8 @@ template <typename T>
 __device__ __forceinline__ void store8(T* p, const float* f) {
     *reinterpret_cast<uint4*>(p) = Vec16<T>::pack(f);
 }
+// relu that keeps NaN (fmaxf(NaN, 0) would return 0); also the backward mask: keep where !(v <= 0)
+__device__ __forceinline__ float relu_nan(float v) { return v <= 0.f ? 0.f : v; }
 
 // ---- bias + relu -------------------------------------------------------------------------------------------------
 template <typename T>
@@ -40,7 +48,7 @@ __global__ void __launch_bounds__(kThreads) bias_relu_fwd_kernel(T* __restrict__
         load8<T>(y + v * 8, a);
         load8<T>(bias + (v % cpv) * 8, b);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) a[k] = fmaxf(a[k] + b[k], 0.f);
+        for (int k = 0; k < 8; ++k) a[k] = relu_nan(a[k] + b[k]);
         store8<T>(y + v * 8, a);
     }
 }
@@ -85,7 +93,7 @@ __global__ void __launch_bounds__(kThreads) bias_relu_bwd_kernel(const T* __rest
             load8<T>(y + off, b);
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                a[k] = b[k] > 0.f ? a[k] : 0.f;
+                a[k] = b[k] <= 0.f ? 0.f : a[k];
                 part[k] += a[k];
             }
             store8<T>(gout + off, a);
@@ -125,11 +133,11 @@ __global__ void __launch_bounds__(kThreads) bias_relu_pool_fwd_kernel(const T* _
             load8<T>(x + base + offs[q], f);
 #pragma unroll
             for (int k = 0; k < 8; ++k)
-                if (f[k] > m[k]) m[k] = f[k], arg[k] = q + 1;
+                if (f[k] > m[k] || f[k] != f[k]) m[k] = f[k], arg[k] = q + 1;
         }
         load8<T>(bias + cv * 8, b);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) m[k] = fmaxf(m[k] + b[k], 0.f);
+        for (int k = 0; k < 8; ++k) m[k] = relu_nan(m[k] + b[k]);
         const size_t o = v * 8;
         store8<T>(out + o, m);
         uint2 packed;
@@ -168,7 +176,7 @@ __global__ void __launch_bounds__(kThreads) bias_relu_pool_bwd_kernel(const T* _
         for (int k = 0; k < 4; ++k) arg[k] = (packed.x >> (8 * k)) & 0xffu, arg[4 + k] = (packed.y >> (8 * k)) & 0xffu;
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
-            a[k] = y[k] > 0.f ? a[k] : 0.f;
+            a[k] = y[k] <= 0.f ? 0.f : a[k];
             part[k] += a[k];
         }
         const size_t base = ((static_cast<size_t>(n) * H + 2 * ho) * W + 2 * wo) * C + cv * 8;
@@ -204,6 +212,12 @@ void check(const char* what) {
 void check_c(int C) {
     if (C % 8 || C > 2048) throw std::runtime_error("bagua: NHWC fused epilogues need C % 8 == 0 and C <= 2048");
 }
+// The kernels access these pointers with 16-byte vectors (the argmax bytes with 8-byte words). A view into a packed buffer (a
+// conv bias after a parameter whose size is not a multiple of 8) can be off by a few bytes; fail here instead of on the device.
+void check_aligned(const char* kernel, const char* arg, const void* p, size_t bytes = 16) {
+    if (reinterpret_cast<uintptr_t>(p) % bytes)
+        throw std::runtime_error(std::string("bagua: ") + kernel + ": `" + arg + "` must be " + std::to_string(bytes) + "-byte aligned");
+}
 int grid_for(size_t items, int multiple_of = 1) {
     size_t b = (items + kThreads - 1) / kThreads;
     const size_t cap = 132 * 8;
@@ -216,6 +230,8 @@ int grid_for(size_t items, int multiple_of = 1) {
 
 void launch_bias_relu_nhwc_fwd(void* y, const void* bias, size_t rows, int C, int dtype, cudaStream_t stream) {
     check_c(C);
+    check_aligned("bias_relu_nhwc_fwd", "y", y);
+    check_aligned("bias_relu_nhwc_fwd", "bias", bias);
     const size_t vecs = rows * C / 8;
     if (!vecs) return;
     dispatch_half(dtype, [&](auto tag) {
@@ -228,6 +244,9 @@ void launch_bias_relu_nhwc_fwd(void* y, const void* bias, size_t rows, int C, in
 void launch_bias_relu_nhwc_bwd(const void* g, const void* y, void* gout, float* bias_grad, size_t rows, int C, int dtype, cudaStream_t stream,
                                void* bias_grad_out, unsigned int* ticket) {
     check_c(C);
+    check_aligned("bias_relu_nhwc_bwd", "g", g);
+    check_aligned("bias_relu_nhwc_bwd", "y", y);
+    check_aligned("bias_relu_nhwc_bwd", "gout", gout);
     if (!rows) return;
     const int cpv = C / 8;
     if (cpv > kThreads) throw std::runtime_error("bagua: bias_relu_nhwc_bwd needs C <= 2048");
@@ -250,6 +269,10 @@ void launch_bias_relu_pool_nhwc_fwd(const void* x, const void* bias, void* out, 
                                     cudaStream_t stream) {
     check_c(C);
     if (H % 2 || W % 2) throw std::runtime_error("bagua: fused max-pool needs even H and W");
+    check_aligned("bias_relu_pool_nhwc_fwd", "x", x);
+    check_aligned("bias_relu_pool_nhwc_fwd", "bias", bias);
+    check_aligned("bias_relu_pool_nhwc_fwd", "out", out);
+    check_aligned("bias_relu_pool_nhwc_fwd", "idx", idx, 8);
     const size_t vecs = static_cast<size_t>(N) * (H / 2) * (W / 2) * (C / 8);
     if (!vecs) return;
     dispatch_half(dtype, [&](auto tag) {
@@ -265,6 +288,10 @@ void launch_bias_relu_pool_nhwc_bwd(const void* g, const void* out, const uint8_
     check_c(C);
     const int cpv = C / 8;
     if (kThreads % cpv) throw std::runtime_error("bagua: fused max-pool backward needs C/8 to divide 256");
+    check_aligned("bias_relu_pool_nhwc_bwd", "g", g);
+    check_aligned("bias_relu_pool_nhwc_bwd", "out", out);
+    check_aligned("bias_relu_pool_nhwc_bwd", "idx", idx, 8);
+    check_aligned("bias_relu_pool_nhwc_bwd", "gin", gin);
     const size_t vecs = static_cast<size_t>(N) * (H / 2) * (W / 2) * cpv;
     if (!vecs) return;
     dispatch_half(dtype, [&](auto tag) {

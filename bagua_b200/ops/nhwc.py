@@ -12,11 +12,25 @@ from ..core import dtype_code, native
 __all__ = ["bias_relu", "bias_relu_maxpool2", "conv_bias_relu", "fused_supported"]
 
 
+def _aligned(t: torch.Tensor) -> bool:
+    """The kernels read and write every tensor with 16-byte vectors."""
+    return t.data_ptr() % 16 == 0
+
+
 def fused_supported(x: torch.Tensor, channels: int) -> bool:
     """Whether the fused NHWC epilogue kernels accept ``x``: channels_last f16/bf16 CUDA 4-D tensor, channels a multiple of 8 that
-    maps onto a 256-thread block (``256 % (channels / 8) == 0``), at most 2048."""
+    maps onto a 256-thread block (``256 % (channels / 8) == 0``), at most 2048, data 16-byte aligned."""
     return (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16) and x.dim() == 4 and channels % 8 == 0 and channels <= 2048
-            and 256 % (channels // 8) == 0 and x.is_contiguous(memory_format=torch.channels_last))
+            and 256 % (channels // 8) == 0 and x.is_contiguous(memory_format=torch.channels_last) and _aligned(x))
+
+
+def _kernel_bias(bias: torch.Tensor) -> torch.Tensor:
+    """``bias`` as the kernels read it: contiguous and 16-byte aligned. A bias that lives in a flattened bucket right after a
+    tensor whose size is not a multiple of 8 is a misaligned view; it is copied (at most 2048 elements), and the copy's gradient
+    flows back into the view."""
+    if bias.is_contiguous() and _aligned(bias):
+        return bias
+    return bias.clone(memory_format=torch.contiguous_format)
 
 
 def _stream() -> int:
@@ -141,6 +155,7 @@ def _native_functions():
 def bias_relu(y: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
     """``relu(y + bias[None, :, None, None])`` in place on a channels_last f16/bf16 CUDA tensor (torch ops otherwise)."""
     if fused_supported(y, y.shape[1]) and bias.dtype == y.dtype:
+        bias = _kernel_bias(bias)
         ext = _native_functions()
         if ext is not None:
             return ext.bias_relu(y, bias)
@@ -151,6 +166,7 @@ def bias_relu(y: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
 def bias_relu_maxpool2(x: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
     """``max_pool2d(relu(x + bias), 2, 2)`` in one pass."""
     if fused_supported(x, x.shape[1]) and bias.dtype == x.dtype and x.shape[2] % 2 == 0 and x.shape[3] % 2 == 0:
+        bias = _kernel_bias(bias)
         ext = _native_functions()
         if ext is not None:
             return ext.bias_relu_maxpool2(x, bias)
@@ -172,7 +188,8 @@ def conv_bias_relu(x: torch.Tensor, conv: torch.nn.Conv2d, pool: bool = False) -
     if conv.bias is not None and fused_supported(x, conv.out_channels) and conv.weight.dtype == x.dtype:
         ext = _native_functions()
         if ext is not None and conv.bias.dtype == x.dtype and (not pool or (_out_hw(x, conv)[0] % 2 == 0 and _out_hw(x, conv)[1] % 2 == 0)):
-            return ext.conv_bias_relu(x, conv.weight, conv.bias, list(conv.stride), list(conv.padding), list(conv.dilation), conv.groups, pool)
+            return ext.conv_bias_relu(x, conv.weight, _kernel_bias(conv.bias), list(conv.stride), list(conv.padding), list(conv.dilation), conv.groups,
+                                      pool)
         y = F.conv2d(x, conv.weight, None, conv.stride, conv.padding, conv.dilation, conv.groups)
         return bias_relu_maxpool2(y, conv.bias) if pool else bias_relu(y, conv.bias)
     y = F.relu(conv(x))

@@ -1,6 +1,7 @@
 // Host test double of the kernel table behind the C++ NHWC autograd Functions (csrc/torch_hooks/nhwc_functions.cpp): lets the
 // CPU suite exercise the Function plumbing (saved tensors, in-place output, shapes, memory format, dtype of the bias gradient,
-// workspace / ticket handling) without a GPU. bf16 only; arithmetic in float.
+// workspace / ticket handling) without a GPU. bf16 only; arithmetic in float. Same NaN rule as the kernels: relu(NaN) = NaN, the
+// gradient is kept where !(y <= 0), and the pool's argmax is the first maximum in scan order or else the last NaN of the window.
 #include <cstdint>
 #include <cstring>
 #include <vector>
@@ -18,6 +19,7 @@ uint16_t f2bf(float f) {
     u += 0x7FFFu + ((u >> 16) & 1u);  // round to nearest even
     return static_cast<uint16_t>(u >> 16);
 }
+float relu(float v) { return v <= 0.f ? 0.f : v; }
 int calls[4] = {0, 0, 0, 0};
 
 int bias_relu_fwd(void* y, const void* bias, size_t rows, int C, int, void*) {
@@ -26,7 +28,7 @@ int bias_relu_fwd(void* y, const void* bias, size_t rows, int C, int, void*) {
     for (size_t r = 0; r < rows; ++r)
         for (int c = 0; c < C; ++c) {
             float v = bf2f(p[r * C + c]) + bf2f(b[c]);
-            p[r * C + c] = f2bf(v > 0.f ? v : 0.f);
+            p[r * C + c] = f2bf(relu(v));
         }
     ++calls[0];
     return 0;
@@ -43,7 +45,7 @@ int bias_relu_bwd(const void* g, const void* y, void* gout, float* bias_grad, si
     auto* po = static_cast<uint16_t*>(gout);
     for (size_t r = 0; r < rows; ++r)
         for (int c = 0; c < C; ++c) {
-            float v = bf2f(py[r * C + c]) > 0.f ? bf2f(pg[r * C + c]) : 0.f;
+            float v = bf2f(py[r * C + c]) <= 0.f ? 0.f : bf2f(pg[r * C + c]);
             po[r * C + c] = f2bf(v);
             bias_grad[c] += v;
         }
@@ -60,16 +62,16 @@ int pool_fwd(const void* x, const void* bias, void* out, uint8_t* idx, int N, in
         for (int ho = 0; ho < Ho; ++ho)
             for (int wo = 0; wo < Wo; ++wo)
                 for (int c = 0; c < C; ++c) {
-                    float best = -3.4e38f;
+                    float best = 0.f;
                     int arg = 0;
                     for (int q = 0; q < 4; ++q) {
                         const int h = 2 * ho + q / 2, w = 2 * wo + q % 2;
                         const float v = bf2f(px[((static_cast<size_t>(n) * H + h) * W + w) * C + c]);
-                        if (v > best) best = v, arg = q;
+                        if (q == 0 || v > best || v != v) best = v, arg = q;
                     }
                     const size_t o = ((static_cast<size_t>(n) * Ho + ho) * Wo + wo) * C + c;
                     const float v = best + bf2f(b[c]);
-                    po[o] = f2bf(v > 0.f ? v : 0.f);
+                    po[o] = f2bf(relu(v));
                     idx[o] = static_cast<uint8_t>(arg);
                 }
     ++calls[2];
@@ -87,7 +89,7 @@ int pool_bwd(const void* g, const void* out, const uint8_t* idx, void* gin, floa
             for (int wo = 0; wo < Wo; ++wo)
                 for (int c = 0; c < C; ++c) {
                     const size_t o = ((static_cast<size_t>(n) * Ho + ho) * Wo + wo) * C + c;
-                    const float v = bf2f(po[o]) > 0.f ? bf2f(pg[o]) : 0.f;
+                    const float v = bf2f(po[o]) <= 0.f ? 0.f : bf2f(pg[o]);
                     const int q = idx[o], h = 2 * ho + q / 2, w = 2 * wo + q % 2;
                     pi[((static_cast<size_t>(n) * H + h) * W + w) * C + c] = f2bf(v);
                     bias_grad[c] += v;

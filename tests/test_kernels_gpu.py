@@ -191,14 +191,15 @@ def test_tcgen05_grouped_gemm_matches_fp32_reference(dev, G, M, N, K):
         torch.testing.assert_close(got.float(), want, rtol=3e-2, atol=3e-2 * want.abs().max().item())
 
 
-@pytest.mark.parametrize("C,H", [(64, 16), (128, 12), (512, 8)])
-def test_fused_nhwc_conv_epilogues_match_torch(dev, C, H):
+@pytest.mark.parametrize("C,H,dtype", [pytest.param(C, H, dt, id=f"{C}-{H}" + ("" if dt == torch.bfloat16 else "-fp16"))
+                                         for dt in (torch.bfloat16, torch.float16) for C, H in [(64, 16), (128, 12), (512, 8)]])
+def test_fused_nhwc_conv_epilogues_match_torch(dev, C, H, dtype):
     from bagua_b200.ops.nhwc import bias_relu, bias_relu_maxpool2
 
     torch.manual_seed(6)
     for pool in (False, True):
-        x = torch.randn(4, C, H, H, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
-        b = torch.randn(C, device=dev).to(torch.bfloat16)
+        x = torch.randn(4, C, H, H, device=dev).to(dtype).contiguous(memory_format=torch.channels_last)
+        b = torch.randn(C, device=dev).to(dtype)
         gy = None
         outs = []
         for fused in (True, False):
@@ -223,18 +224,19 @@ def test_fused_nhwc_conv_epilogues_match_torch(dev, C, H):
 def test_vgg16_fused_path_matches_module_path(dev):
     from bagua_b200.models import vgg16
 
-    torch.manual_seed(8)
-    m = vgg16(num_classes=10).to(dev).to(torch.bfloat16).to(memory_format=torch.channels_last).eval()
-    x = torch.randn(2, 3, 64, 64, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
-    res = []
-    for fuse in (True, False):
-        m.fuse_epilogues = fuse
-        m.zero_grad()
-        out = m(x)
-        out.float().sum().backward()
-        res.append((out.detach().float(), m.features[0].bias.grad.float().clone(), m.features[28].weight.grad.float().clone()))
-    for a, b in zip(*res):
-        torch.testing.assert_close(a, b, rtol=5e-2, atol=5e-2 * max(1.0, b.abs().max().item()))
+    for dtype in (torch.bfloat16, torch.float16):
+        torch.manual_seed(8)
+        m = vgg16(num_classes=10).to(dev).to(dtype).to(memory_format=torch.channels_last).eval()
+        x = torch.randn(2, 3, 64, 64, device=dev).to(dtype).contiguous(memory_format=torch.channels_last)
+        res = []
+        for fuse in (True, False):
+            m.fuse_epilogues = fuse
+            m.zero_grad()
+            out = m(x)
+            out.float().sum().backward()
+            res.append((out.detach().float(), m.features[0].bias.grad.float().clone(), m.features[28].weight.grad.float().clone()))
+        for a, b in zip(*res):
+            torch.testing.assert_close(a, b, rtol=5e-2, atol=5e-2 * max(1.0, b.abs().max().item()))
 
 
 @pytest.mark.parametrize("pool", [False, True])
