@@ -289,6 +289,17 @@ PYBIND11_MODULE(_C, m) {
             .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, int, uint64_t, bool, LaunchCfg>(),
                  py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("master_ptr"), py::arg("exp_avg_ptr"),
                  py::arg("exp_avg_sq_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("ratio_ptr"), py::arg("use_multimem"), py::arg("cfg")));
+    def_stepped<LarsNormsOp, float, float, float, float>(
+        py::class_<LarsNormsOp, CommOp, std::shared_ptr<LarsNormsOp>>(m, "LarsNormsOp")
+            .def(py::init<uint64_t, uint64_t, uint64_t, uint64_t, int, int, int, uint64_t, uint64_t>(), py::arg("ptrs"), py::arg("sizes"), py::arg("b2t"),
+                 py::arg("b2c"), py::arg("n_tensors"), py::arg("n_blocks"), py::arg("chunk"), py::arg("coef_ptr"), py::arg("partials_ptr")));
+    def_stepped<ShardLarsOp, float, float, float, float>(
+        py::class_<ShardLarsOp, CommOp, std::shared_ptr<ShardLarsOp>>(m, "ShardLarsOp")
+            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, uint64_t, int, uint64_t, bool,
+                          LaunchCfg>(),
+                 py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
+                 py::arg("master_ptr"), py::arg("momentum_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("sums_ptr"), py::arg("use_multimem"),
+                 py::arg("cfg")));
     py::class_<PeerAverageOp, CommOp, std::shared_ptr<PeerAverageOp>>(m, "PeerAverageOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, uint64_t, size_t, int, LaunchCfg>(), py::arg("comm"), py::arg("weights"),
              py::arg("off"), py::arg("out_ptr"), py::arg("bytes"), py::arg("dtype"), py::arg("cfg"))
@@ -387,6 +398,21 @@ PYBIND11_MODULE(_C, m) {
               TensorListDesc d{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes),
                                reinterpret_cast<const int32_t*>(b2t), reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk};
               launch_multi_tensor_lamb_stage2(d, dtype, mixed, lamb_params(lr, b1, b2, eps, wd, step), reinterpret_cast<const double*>(sums), S(stream));
+          });
+    m.def("multi_tensor_lars_stage1",
+          [](uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, int dtype, bool mixed, uint64_t coef,
+             uint64_t sums, uint64_t stream) {
+              TensorListDesc d{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes),
+                               reinterpret_cast<const int32_t*>(b2t), reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk};
+              launch_multi_tensor_lars_stage1(d, dtype, mixed, reinterpret_cast<const float*>(coef), reinterpret_cast<double*>(sums), S(stream));
+          });
+    m.def("multi_tensor_lars_stage2",
+          [](uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, int dtype, bool mixed, float lr,
+             float momentum, float wd, float trust_coefficient, uint64_t coef, uint64_t sums, bool zero_grad, uint64_t stream) {
+              TensorListDesc d{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes),
+                               reinterpret_cast<const int32_t*>(b2t), reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk};
+              launch_multi_tensor_lars_stage2(d, dtype, mixed, LarsParams{lr, momentum, wd, trust_coefficient}, reinterpret_cast<const float*>(coef),
+                                              reinterpret_cast<const double*>(sums), zero_grad, S(stream));
           });
     m.def("qadam_momentum", [](uint64_t m1, uint64_t grad, int gdt, size_t n, float beta1, uint64_t stream) {
         launch_qadam_momentum(reinterpret_cast<float*>(m1), reinterpret_cast<const void*>(grad), gdt, n, beta1, S(stream));

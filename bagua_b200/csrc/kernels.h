@@ -46,6 +46,15 @@ struct LambParams {
     float bias_correction2;  // 1 - beta2^t
 };
 
+// LARS (You et al. 2017, the MLPerf ResNet-50 form): trust = trust_coefficient·‖w‖/(‖g̃‖ + wd·‖w‖) per parameter where
+// weight_decay != 0, momentum buffer v ← μ·v + lr·trust·(g̃ + wd·w), w ← w − v (see lars.cuh). No step-dependent field.
+struct LarsParams {
+    float lr;
+    float momentum;
+    float weight_decay;
+    float trust_coefficient;
+};
+
 // 1 - beta^step of the in-bucket Adam and LAMB ops and of FusedLAMB: in double, rounded once. Also callable from device code: the
 // kernels that take the step count from device memory (loss scaling) build their bias corrections with it.
 #ifdef __CUDACC__
@@ -115,6 +124,14 @@ void launch_lamb_ratio(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, c
 void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, float* master, const float* exp_avg,
                        const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, const LambParams& hp, bool use_multimem,
                        int nblocks, int nthreads, cudaStream_t stream, const float* vote = nullptr, const uint32_t* step = nullptr);
+// In-bucket LARS, the same program as LAMB: launch_multi_tensor_lars_stage1 over the shard's segments ([master, gradient shard]
+// lists) leaves fp64 {Σw², Σg̃²} per block, launch_lamb_ratio exchanges them per parameter (its `ratio` output goes unused) into
+// sums[2t], sums[2t+1], and shard_lars applies the update to the owned slice with trust = lars_trust(sums of segs[3s+2]) for the
+// elements [segs[3s], segs[3s+1]) (1 in the gaps), g̃ = shard·*coef (coef nullable = 1), then all-gathers the weights. `vote`: coef
+// addresses {coef, found_inf} and a found_inf step goes straight to the closing barrier.
+void launch_shard_lars(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                       float* master, float* momentum, const int32_t* segs, int nsegs, const double* sums, const LarsParams& hp, bool use_multimem,
+                       int nblocks, int nthreads, cudaStream_t stream, bool vote = false);
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,
                          int nblocks, int nthreads, cudaStream_t stream);
 void launch_peer_barrier(const PeerCtx& ctx, cudaStream_t stream);
@@ -247,6 +264,14 @@ void launch_multi_tensor_sgd_mp(const TensorListDesc& d, int dtype, bool has_mom
 void launch_multi_tensor_lamb_stage1(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const float* coef, double* sums, bool zero_grad,
                                      cudaStream_t stream, const uint32_t* step = nullptr);
 void launch_multi_tensor_lamb_stage2(const TensorListDesc& d, int dtype, bool mixed, const LambParams& hp, const double* sums, cudaStream_t stream);
+// LARS in two launches, lists [param(T), grad(T), momentum(f32)(, master(f32) when mixed)]. Stage 1: fp64 {Σw², Σg̃²} of each block
+// in sums[2·block] with g̃ = grad·*coef (coef nullable = 1); it reads lists 0, 1 (and the master) only and never clears the gradient.
+// With `vote` coef addresses {coef, found_inf} and a found_inf step writes nothing. Stage 2: each block sums its tensor's block
+// partials in a fixed order, forms the trust (lars.cuh) and applies the momentum and the update with the same g̃; mixed writes the
+// fp32 master and the parameter rounded once; the gradient is cleared when zero_grad.
+void launch_multi_tensor_lars_stage1(const TensorListDesc& d, int dtype, bool mixed, const float* coef, double* sums, cudaStream_t stream, bool vote = false);
+void launch_multi_tensor_lars_stage2(const TensorListDesc& d, int dtype, bool mixed, const LarsParams& hp, const float* coef, const double* sums, bool zero_grad,
+                                     cudaStream_t stream);
 // QAdam momentum pre-step (bagua/torch_api/algorithms/q_adam.py:193-221): m = beta1*m + (1-beta1)*g
 void launch_qadam_momentum(float* exp_avg, const void* grad, int grad_dtype, size_t numel, float beta1, cudaStream_t stream);
 

@@ -12,6 +12,7 @@
 #include "dispatch.h"
 #include "kernels.h"
 #include "lamb.cuh"
+#include "lars.cuh"
 #include "quant.cuh"
 
 namespace bagua {
@@ -463,6 +464,111 @@ void launch_multi_tensor_lamb_stage2(const TensorListDesc& d, int dtype, bool mi
             multi_tensor_lamb_stage2_kernel<T, false><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, sums);
     });
     check_launch("multi_tensor_lamb_stage2");
+}
+
+// ---- LARS: per-block norms, then per-tensor trust + momentum + apply -------------------------------------------
+// The block layout of the LAMB kernels above: stage 1 leaves one fp64 {Σw², Σg̃²} pair per block (no atomics, the gradient left in
+// place for stage 2), stage 2 adds its tensor's block pairs in block order and recomputes g̃ with the same lars_grad.
+// VOTE (the in-bucket LARS with loss scaling): coef addresses {coef, found_inf}; a skipped step returns before any write.
+template <typename T, bool MIXED, bool VOTE>
+__global__ void __launch_bounds__(kThreads) multi_tensor_lars_stage1_kernel(TensorListDesc d, const float* coef, double* sums) {
+    __shared__ double s_w[kThreads / 32], s_g[kThreads / 32];
+    if constexpr (VOTE) {
+        if (coef[1] != 0.f) return;
+    }
+    const int t = d.block_to_tensor[blockIdx.x];
+    const size_t off = static_cast<size_t>(d.block_to_chunk[blockIdx.x]) * d.chunk;
+    const size_t n = static_cast<size_t>(d.sizes[t]);
+    const size_t len = (n - off) < static_cast<size_t>(d.chunk) ? (n - off) : static_cast<size_t>(d.chunk);
+    const T* p = reinterpret_cast<const T*>(d.ptrs[t]) + off;
+    const T* g = reinterpret_cast<const T*>(d.ptrs[d.n_tensors + t]) + off;
+    const float* mw = MIXED ? reinterpret_cast<const float*>(d.ptrs[3 * d.n_tensors + t]) + off : nullptr;
+    const float c = coef != nullptr ? *coef : 1.f;
+    double sw = 0.0, sg = 0.0;
+    for (size_t i = threadIdx.x; i < len; i += blockDim.x) {
+        const float w = MIXED ? mw[i] : to_f32<T>(p[i]);
+        const float gt = lars_grad(to_f32<T>(g[i]), c);
+        sw += static_cast<double>(w) * static_cast<double>(w);
+        sg += static_cast<double>(gt) * static_cast<double>(gt);
+    }
+    // fixed order: a shuffle tree per warp, then the warps in index order
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        sw += __shfl_xor_sync(0xffffffffu, sw, o);
+        sg += __shfl_xor_sync(0xffffffffu, sg, o);
+    }
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = sw, s_g[threadIdx.x >> 5] = sg;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double a = 0.0, b = 0.0;
+        for (unsigned k = 0; k < blockDim.x / 32; ++k) a += s_w[k], b += s_g[k];
+        sums[2 * blockIdx.x] = a;
+        sums[2 * blockIdx.x + 1] = b;
+    }
+}
+
+template <typename T, bool MIXED>
+__global__ void __launch_bounds__(kThreads)
+    multi_tensor_lars_stage2_kernel(TensorListDesc d, LarsParams hp, const float* coef, const double* sums, int zero_grad) {
+    __shared__ float s_trust;
+    const int t = d.block_to_tensor[blockIdx.x];
+    const int chunk_idx = d.block_to_chunk[blockIdx.x];
+    const size_t off = static_cast<size_t>(chunk_idx) * d.chunk;
+    const size_t n = static_cast<size_t>(d.sizes[t]);
+    const size_t len = (n - off) < static_cast<size_t>(d.chunk) ? (n - off) : static_cast<size_t>(d.chunk);
+    if (threadIdx.x < 32) {  // the tensor's blocks are consecutive from blockIdx.x − chunk_idx: one warp adds their pairs in a fixed order
+        const int first = blockIdx.x - chunk_idx;
+        const int nb = static_cast<int>((n + d.chunk - 1) / d.chunk);
+        double a = 0.0, b = 0.0;
+        for (int k = threadIdx.x; k < nb; k += 32) a += sums[2 * (first + k)], b += sums[2 * (first + k) + 1];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            a += __shfl_xor_sync(0xffffffffu, a, o);
+            b += __shfl_xor_sync(0xffffffffu, b, o);
+        }
+        if (threadIdx.x == 0) s_trust = lars_trust(a, b, hp);
+    }
+    __syncthreads();
+    const float lt = lars_step_size(s_trust, hp);
+    const float c = coef != nullptr ? *coef : 1.f;
+    T* p = reinterpret_cast<T*>(d.ptrs[t]) + off;
+    T* g = reinterpret_cast<T*>(d.ptrs[d.n_tensors + t]) + off;
+    float* mo = reinterpret_cast<float*>(d.ptrs[2 * d.n_tensors + t]) + off;
+    float* mw = MIXED ? reinterpret_cast<float*>(d.ptrs[3 * d.n_tensors + t]) + off : nullptr;
+    for (size_t i = threadIdx.x; i < len; i += blockDim.x) {
+        float w = MIXED ? mw[i] : to_f32<T>(p[i]), v = mo[i];
+        lars_apply(w, v, lars_grad(to_f32<T>(g[i]), c), lt, hp);
+        mo[i] = v;
+        if (MIXED) mw[i] = w;
+        p[i] = from_f32<T>(w);
+        if (zero_grad) g[i] = from_f32<T>(0.f);
+    }
+}
+
+void launch_multi_tensor_lars_stage1(const TensorListDesc& d, int dtype, bool mixed, const float* coef, double* sums, cudaStream_t stream, bool vote) {
+    if (d.n_blocks <= 0) return;
+    if (vote && coef == nullptr) throw std::runtime_error("bagua: multi_tensor_lars_stage1 with a vote needs {coef, found_inf}");
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
+        using T = decltype(tag);
+        dispatch_flag(mixed, [&](auto mx) {
+            dispatch_flag(vote, [&](auto vt) {
+                multi_tensor_lars_stage1_kernel<T, decltype(mx)::value, decltype(vt)::value><<<d.n_blocks, kThreads, 0, stream>>>(d, coef, sums);
+            });
+        });
+    });
+    check_launch("multi_tensor_lars_stage1");
+}
+
+void launch_multi_tensor_lars_stage2(const TensorListDesc& d, int dtype, bool mixed, const LarsParams& hp, const float* coef, const double* sums, bool zero_grad,
+                                     cudaStream_t stream) {
+    if (d.n_blocks <= 0) return;
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
+        using T = decltype(tag);
+        dispatch_flag(mixed, [&](auto mx) {
+            multi_tensor_lars_stage2_kernel<T, decltype(mx)::value><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, coef, sums, zero_grad ? 1 : 0);
+        });
+    });
+    check_launch("multi_tensor_lars_stage2");
 }
 
 // ---- QAdam momentum pre-step -------------------------------------------------------------------------------------

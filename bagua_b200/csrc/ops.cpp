@@ -205,6 +205,19 @@ void ShardLambOp::run(Bucket&, StreamHandle stream, int) {
     steps_++;
 }
 
+void LarsNormsOp::run(Bucket&, StreamHandle stream, int) {
+    launch_multi_tensor_lars_stage1(desc_, F32, false, coef_or_vote(coef_), reinterpret_cast<double*>(partials_), S(stream), vote() != nullptr);
+    steps_++;
+}
+
+void ShardLarsOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("shard_lars");
+    launch_shard_lars(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), coef_or_vote(coef_),
+                      reinterpret_cast<float*>(master_), reinterpret_cast<float*>(momentum_), reinterpret_cast<const int32_t*>(segs_), nsegs_,
+                      reinterpret_cast<const double*>(sums_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream), vote() != nullptr);
+    steps_++;
+}
+
 int PeerAverageOp::shift_one_peer(int rank, int nranks, int64_t step) {
     const int64_t r = rank, n = nranks;
     if (rank < nranks / 2) return static_cast<int>(((step + r) % ((n + 1) / 2)) + (n / 2));

@@ -127,6 +127,9 @@ struct AdamHyper {
 struct LambHyper {
     float lr = 1e-3f, beta1 = 0.9f, beta2 = 0.999f, eps = 1e-6f, weight_decay = 0.01f;
 };
+struct LarsHyper {
+    float lr = 1e-3f, momentum = 0.9f, weight_decay = 0.f, trust_coefficient = 1e-3f;
+};
 
 // What a rule's kernel receives at the launch that follows `steps` earlier ones.
 inline SgdParams device_params(const SgdHyper& h, uint64_t steps) {
@@ -136,6 +139,7 @@ inline AdamParams device_params(const AdamHyper& h, uint64_t steps) {
     return adam_params(h.lr, h.beta1, h.beta2, h.eps, h.weight_decay, h.adamw, steps + 1);
 }
 inline LambParams device_params(const LambHyper& h, uint64_t steps) { return lamb_params(h.lr, h.beta1, h.beta2, h.eps, h.weight_decay, steps + 1); }
+inline LarsParams device_params(const LarsHyper& h, uint64_t) { return LarsParams{h.lr, h.momentum, h.weight_decay, h.trust_coefficient}; }
 
 // An optimizer op: hyper-parameters published from Python (the forward pre-hook may do so while the comm worker runs the op, hence
 // the lock) and the count of launches so far, which checkpoints save and restore. With loss scaling a launch may be a skipped step,
@@ -421,6 +425,45 @@ private:
     uint64_t master_, m1_, m2_, segs_;
     int nsegs_;
     uint64_t ratio_;
+    bool use_mc_;
+    LaunchCfg cfg_;
+};
+
+// In-bucket LARS, run from step() after phase A like LAMB: LarsNormsOp per bucket (the multi-tensor LARS stage 1 over the shard's
+// segment table, lists [fp32 master, gradient shard]: fp64 {Σw², Σg̃²} per block into `partials`, g̃ = shard·*coef), the LAMB
+// ratio exchange (LambRatioOp) once per step for the per-parameter global sums, ShardLarsOp per bucket (momentum + apply from the
+// exchanged sums, all-gather, barrier). The rule has no step-dependent parameter; both ops count their launches for checkpoints.
+class LarsNormsOp final : public SteppedOp<LarsHyper> {
+public:
+    LarsNormsOp(uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, uint64_t coef, uint64_t partials)
+        : desc_{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes), reinterpret_cast<const int32_t*>(b2t),
+                reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk},
+          coef_(coef), partials_(partials) {}
+    const char* kind() const override { return "lars_norms"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+
+private:
+    TensorListDesc desc_;
+    uint64_t coef_, partials_;
+};
+
+class ShardLarsOp final : public SteppedOp<LarsHyper> {
+public:
+    ShardLarsOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
+                uint64_t momentum, uint64_t segs, int nsegs, uint64_t sums, bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), master_(master),
+          momentum_(momentum), segs_(segs), nsegs_(nsegs), sums_(sums), use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return "shard_lars"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf weights_;
+    size_t w_off_, bytes_;
+    int dtype_;
+    uint64_t shard_, coef_, master_, momentum_, segs_;
+    int nsegs_;
+    uint64_t sums_;
     bool use_mc_;
     LaunchCfg cfg_;
 };

@@ -7,6 +7,7 @@
 #include "dispatch.h"
 #include "kernels.h"
 #include "lamb.cuh"
+#include "lars.cuh"
 #include "peer.cuh"
 
 namespace bagua {
@@ -665,6 +666,53 @@ __global__ void __launch_bounds__(512) shard_lamb_kernel(PeerCtx ctx, PeerBuf we
     store_epoch(ctx, e0 + 1);
 }
 
+// In-bucket LARS, the program of LAMB with a different pair: multi_tensor_lars_stage1 over the shard's segments leaves fp64
+// {Σw², Σg̃²} per block, lamb_ratio_kernel exchanges them per parameter into sums (its ratio output goes unused), and this kernel
+// applies momentum and update to the owned slice from the gradient shard·coef (lars_grad, the code that fed Σg̃²), then all-gathers
+// the weights and takes the closing barrier. The trust of an element's parameter comes from the exchanged global sums and is taken
+// again only when the walk enters another parameter (1 in the gaps of the segment table). VOTE: coef addresses {coef, found_inf};
+// a skipped step goes straight to the closing barrier.
+template <typename T, int P, bool USE_MC, bool VOTE>
+__global__ void __launch_bounds__(512) shard_lars_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
+                                                         const float* coef, float* master, float* momentum, const int32_t* segs, int nsegs,
+                                                         const double* sums, LarsParams hp) {
+    const uint32_t e0 = load_epoch(ctx);
+    constexpr int N = Vec16<T>::N;
+    const float c = coef != nullptr ? *coef : 1.f;
+    bool skip = false;
+    if constexpr (VOTE) skip = coef[1] != 0.f;
+    if (!skip) {
+        int cur = -2;    // parameter whose step size lt holds (−1: a gap)
+        float lt = 0.f;
+        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard, [&](size_t j, const float* g, float* w) {
+            float4* mp = reinterpret_cast<float4*>(master + j * N);
+            float4* vp = reinterpret_cast<float4*>(momentum + j * N);
+            int s = lamb_segment_at(segs, nsegs, static_cast<int64_t>(j * N));
+#pragma unroll
+            for (int q = 0; q < N / 4; ++q) {
+                const float4 ww = mp[q], vv = vp[q];
+                float wv[4] = {ww.x, ww.y, ww.z, ww.w}, v[4] = {vv.x, vv.y, vv.z, vv.w};
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const int64_t e = static_cast<int64_t>(j * N + 4 * q + k);
+                    while (s + 1 < nsegs && segs[3 * (s + 1)] <= e) ++s;
+                    const int t = (s >= 0 && e < segs[3 * s + 1]) ? segs[3 * s + 2] : -1;
+                    if (t != cur) {
+                        cur = t;
+                        lt = lars_step_size(t >= 0 ? lars_trust(sums[2 * t], sums[2 * t + 1], hp) : 1.f, hp);
+                    }
+                    lars_apply(wv[k], v[k], lars_grad(g[4 * q + k], c), lt, hp);
+                    w[4 * q + k] = wv[k];
+                }
+                mp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
+                vp[q] = make_float4(v[0], v[1], v[2], v[3]);
+            }
+        });
+    }
+    peer_barrier(ctx, e0 + 1);
+    store_epoch(ctx, e0 + 1);
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Decentralized SGD, shift_one: out = (mine + peer's weights) / 2, the peer's bucket being read straight over
 // NVLink (replaces grouped send/recv + average kernel, comm_ops/decentralized_full_precision_synchronous.rs:81-92).
@@ -1056,6 +1104,25 @@ void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off,
         });
     });
     check_launch("shard_lamb");
+}
+
+void launch_shard_lars(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                       float* master, float* momentum, const int32_t* segs, int nsegs, const double* sums, const LarsParams& hp, bool use_multimem,
+                       int nblocks, int nthreads, cudaStream_t stream, bool vote) {
+    const size_t vecs = peer_vecs("shard_lars", bytes, w_off, 0, nblocks);
+    if (vote && coef == nullptr) throw std::runtime_error("bagua: shard_lars with a vote needs {coef, found_inf}");
+    if (vecs == 0) return;
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(ctx.world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                dispatch_flag(vote, [&](auto vt) {
+                    shard_lars_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(vt)::value><<<nblocks, nthreads, 0, stream>>>(
+                        ctx, weights, w_off, vecs, shard, coef, master, momentum, segs, nsegs, sums, hp);
+                });
+            });
+        });
+    });
+    check_launch("shard_lars");
 }
 
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,

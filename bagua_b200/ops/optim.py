@@ -16,7 +16,7 @@ import torch
 from ..core import dtype_code, native
 from ..tensor import dense_strides
 
-__all__ = ["FusedSGD", "FusedAdam", "FusedLAMB", "flat_sgd_", "flat_adam_", "multi_tensor_plan"]
+__all__ = ["FusedSGD", "FusedAdam", "FusedLAMB", "FusedLARS", "flat_sgd_", "flat_adam_", "multi_tensor_plan"]
 
 
 def _stream() -> int:
@@ -613,3 +613,95 @@ class FusedLAMB(_FusedBase):
                 if wn > 0 and un > 0:
                     r = float(torch.tensor(wn / un, dtype=torch.float32))
             p.data.copy_(w - (lr * r) * u)
+
+
+class FusedLARS(_FusedBase):
+    """LARS with layer-wise trust ratios (You et al., 2017, "Large Batch Training of Convolutional Networks"; the MLPerf
+    ResNet-50 form), two multi-tensor kernels per (dtype) group and step.
+
+    ``trust = trust_coefficient·‖w‖ / (‖g‖ + wd·‖w‖)`` over each whole parameter when ``wd ≠ 0`` and both norms are positive
+    (fp64 sums, one rounding to fp32), NaN when a sum is NaN, else 1 — so a ``weight_decay=0`` group (biases, BatchNorm) gets
+    plain momentum SGD; then ``v ← μ·v + (lr·trust)·(g + wd·w)``, ``w ← w − v``. No epsilon, Nesterov or dampening.
+
+    The momentum buffer holds the lr-scaled step, as in the MLPerf reference. ``torch.optim.SGD`` keeps the unscaled one
+    (``v ← μ·v + d``, ``w ← w − lr·v``); the two agree at a constant ``lr`` and differ whenever ``lr`` changes between steps (a
+    warm-up or decay schedule): here an ``lr`` change only affects the new part of the step, there it rescales the whole history.
+
+    On CUDA every step is two multi-tensor kernels per dtype: per-block fp64 ``Σw²``/``Σg²``, then the per-parameter trust (a
+    fixed-order sum of the parameter's block partials) with the momentum and the update. The momentum is fp32;
+    ``master_weights=True`` keeps fp32 master weights for bf16/fp16 parameters and writes the parameter rounded once.
+    ``zero_grad_in_step=True`` clears the gradients in the second kernel. CPU tensors take a torch implementation of the same
+    rule."""
+
+    def __init__(self, params, lr=1e-3, momentum=0.9, weight_decay=0.0, trust_coefficient=1e-3, master_weights=True, zero_grad_in_step=True):
+        defaults = dict(lr=lr, momentum=momentum, weight_decay=weight_decay, trust_coefficient=trust_coefficient)
+        super().__init__(params, defaults, master_weights, zero_grad_in_step)
+        self._sums: Dict[tuple, torch.Tensor] = {}
+
+    @torch.no_grad()
+    def step(self, closure=None, only: Optional[set] = None):
+        """``only``: see :meth:`FusedSGD.step`."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        C = native()
+        for gi, group in enumerate(self.param_groups):
+            lr, mom, wd, eta = group["lr"], group["momentum"], group["weight_decay"], group["trust_coefficient"]
+            params = [p for p in group["params"] if p.grad is not None and (only is None or id(p) in only)]
+            if not params:
+                continue
+            if not _kernels_apply(params):
+                self._torch_step(params, group)
+                continue
+            for p in params:
+                st = self.state[p]
+                buf = st.get("momentum_buffer")
+                if buf is None:   # fp32 momentum in the parameter's memory order (the kernels walk raw memory)
+                    st["momentum_buffer"] = torch.zeros_like(p.data, dtype=torch.float32)
+                elif buf.dtype != torch.float32 or buf.stride() != p.stride():   # e.g. a checkpoint written with another layout
+                    st["momentum_buffer"] = torch.empty_like(p.data, dtype=torch.float32).copy_(buf)
+                if self.master_weights and p.dtype in (torch.float16, torch.bfloat16) and "master" not in st:
+                    st["master"] = torch.empty_like(p.data, dtype=torch.float32).copy_(p.data)
+            for (dt, k), ps in _launch_groups(params, lambda p: 0):
+                mixed = self.master_weights and dt in (torch.float16, torch.bfloat16)
+                grads = [_grad_in_layout(p, dt) for p in ps]
+                lists = [[p.data for p in ps], grads, [self.state[p]["momentum_buffer"] for p in ps]]
+                if mixed:
+                    lists.append([self.state[p]["master"] for p in ps])
+                plan = _cached_plan(self._multi, (gi, dt, k), lists)
+                sums = self._sums.get((gi, dt, k))
+                if sums is None or sums.shape[0] < plan.n_blocks:
+                    sums = self._sums[(gi, dt, k)] = torch.empty(max(plan.n_blocks, 1), 2, dtype=torch.float64, device=ps[0].device)
+                C.multi_tensor_lars_stage1(*plan.args(), dtype_code(dt), mixed, 0, sums.data_ptr(), _stream())
+                C.multi_tensor_lars_stage2(*plan.args(), dtype_code(dt), mixed, float(lr), float(mom), float(wd), float(eta), 0, sums.data_ptr(),
+                                           bool(self.zero_grad_in_step), _stream())
+                self.kernel_launches += 2
+                if self.zero_grad_in_step:
+                    for p, g in zip(ps, grads):
+                        if g is not p.grad:   # the kernel cleared a converted copy
+                            p.grad.zero_()
+        if only is None:
+            self._grads_zeroed = self.zero_grad_in_step
+        return loss
+
+    def _torch_step(self, params, group):
+        """The same rule in torch fp32 (CPU tensors)."""
+        import math
+
+        lr, mom, wd, eta = group["lr"], group["momentum"], group["weight_decay"], group["trust_coefficient"]
+        for p in params:
+            st = self.state[p]
+            if "momentum_buffer" not in st:
+                st["momentum_buffer"] = torch.zeros_like(p.data, dtype=torch.float32)
+            g, w = p.grad.float(), p.data.float()
+            W, G = float(w.double().square().sum()), float(g.double().square().sum())
+            trust = 1.0
+            if math.isnan(W) or math.isnan(G):
+                trust = float("nan")
+            elif wd != 0 and W > 0 and G > 0:
+                trust = eta * math.sqrt(W) / (math.sqrt(G) + wd * math.sqrt(W))
+            lt = float(torch.tensor(lr, dtype=torch.float32) * torch.tensor(trust, dtype=torch.float32))
+            v = st["momentum_buffer"]
+            v.mul_(mom).add_(g + wd * w, alpha=lt)
+            p.data.copy_(w - v)

@@ -53,11 +53,16 @@ class GradientAllReduceAlgorithm(Algorithm):
 # ---------------------------------------------------------------------------------------------------------------
 # Checkpointable state of the in-bucket optimizers
 # ---------------------------------------------------------------------------------------------------------------
-_STATE_KEYS = {"sgd": ("master", "momentum_buffer"), "adam": ("master", "exp_avg", "exp_avg_sq"), "lamb": ("master", "exp_avg", "exp_avg_sq")}
-# what set_hyper of a rule's bucket ops takes, from a parameter group (a LAMB bucket's moments and apply op take the same)
+_STATE_KEYS = {"sgd": ("master", "momentum_buffer"), "adam": ("master", "exp_avg", "exp_avg_sq"), "lamb": ("master", "exp_avg", "exp_avg_sq"),
+               "lars": ("master", "momentum_buffer")}
+# what set_hyper of a rule's bucket ops takes, from a parameter group (a LAMB or LARS bucket's two ops take the same)
 _HYPER = {"sgd": lambda g: (float(g["lr"]), float(g["momentum"]), float(g["dampening"]), float(g["weight_decay"]), bool(g["nesterov"])),
           "adam": lambda g: (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]), bool(g["adamw"])),
-          "lamb": lambda g: (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]))}
+          "lamb": lambda g: (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"])),
+          "lars": lambda g: (float(g["lr"]), float(g["momentum"]), float(g["weight_decay"]), float(g["trust_coefficient"]))}
+# the rules whose trust ratio is a norm over a whole parameter: phase A in the bucket program, then per-bucket norms, one
+# per-parameter exchange and the per-bucket update in step()
+_PER_PARAMETER = ("lamb", "lars")
 
 
 def consolidate_shards(shards, numel: int, layout):
@@ -97,9 +102,9 @@ class _Bucketing:
         self.covered = set()   # ids of the bucketed parameters
         self.uncovered = None  # the parameters outside the buckets, looked up once
         self.clip = None       # the norm exchange shared by all buckets (max_grad_norm and / or loss_scaling), see _clip_state
-        self.lamb = None       # the per-parameter ratio exchange shared by all buckets (LAMB), see _lamb_state
+        self.lamb = None       # the per-parameter exchange shared by all buckets (LAMB and LARS), see _per_param_state
         # the program step() runs after the norm exchange, on the current stream of `device`: every bucket's pre-update op (LAMB
-        # moments), LAMB's ratio exchange, every bucket's update op; empty when the updates run in the bucket kernels
+        # moments, LARS norms), the per-parameter exchange, every bucket's update op; empty when the updates run in the bucket kernels
         self.pre_ops = []
         self.update_ops = []
         self.device = None
@@ -132,9 +137,9 @@ class _ShardedStateMixin:
     @property
     def native_ops_in_step(self) -> bool:
         """Whether ``step()`` runs native kernels once the bucket kernels are live: the norm exchange and the clipped update with
-        ``max_grad_norm`` or ``loss_scaling``, LAMB's moments, ratio exchange and update always. They carry per-call host state
-        (box parity, step count), so such a step cannot be captured in a CUDA graph."""
-        return self.max_grad_norm is not None or self.loss_scaling or self._kind == "lamb"
+        ``max_grad_norm`` or ``loss_scaling``, LAMB's and LARS's per-bucket norms, per-parameter exchange and update always. They carry
+        per-call host state (box parity, step count), so such a step cannot be captured in a CUDA graph."""
+        return self.max_grad_norm is not None or self.loss_scaling or self._kind in _PER_PARAMETER
 
     def _gather(self, t, group):
         import torch
@@ -337,7 +342,7 @@ class _ShardedStateMixin:
             from ...core import native
 
             if b.lamb is not None and b.lamb["ratio_op"] is None:
-                raise RuntimeError("the LAMB ratio exchange was not built: not every bucket of the model has been initialised")
+                raise RuntimeError(f"the {self._kind.upper()} per-parameter exchange was not built: not every bucket of the model has been initialised")
             C, stream, dev = native(), torch.cuda.current_stream(b.device).cuda_stream, b.device.index
             for op in b.pre_ops:
                 C.run_op(op, stream, dev)
@@ -447,6 +452,33 @@ def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weigh
     return opt
 
 
+class ShardedFusedLars(object):
+    """Marker mix-in: see :func:`make_sharded_fused_lars`."""
+
+
+def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, trust_coefficient=1e-3, max_grad_norm=None, loss_scaling=False):
+    """LARS (see :class:`bagua_b200.ops.optim.FusedLARS`) on the in-bucket sharded path: each rank keeps fp32 master weights and
+    the momentum for its 1/N slice of every bucket.
+
+    The trust ratio ``trust_coefficient·‖w‖/(‖g‖ + wd·‖w‖)`` is a norm over a whole parameter, so the program is LAMB's (see
+    :func:`make_sharded_fused_lamb`): each bucket kernel only reduce-scatters the averaged gradient into an fp32 shard, and
+    ``step()`` runs the norm exchange when ``max_grad_norm`` or ``loss_scaling`` is set, the fp64 partial ``Σw²``/``Σg²`` of every
+    shard per parameter segment, one exchange of the per-parameter sums between the ranks (every rank obtains the same bits), and
+    the momentum, the update and the all-gather of the weights per bucket — ``2·buckets + 1`` launches (+1 with the norm
+    exchange). The gradient the norms and the update see is the clipped / unscaled one. Put parameters with ``ndim ≤ 1``
+    (biases, BatchNorm) in a ``weight_decay=0`` group: they get plain momentum SGD. With one process, or without a peer engine, it
+    behaves like :class:`bagua_b200.ops.optim.FusedLARS`; ``loss_scaling``: see :func:`make_sharded_fused_sgd`."""
+    from ...ops.optim import FusedLARS
+
+    class _ShardedFusedLars(_ShardedStateMixin, FusedLARS, ShardedFusedLars):
+        _kind = "lars"
+
+    opt = _ShardedFusedLars(params, lr=lr, momentum=momentum, weight_decay=weight_decay, trust_coefficient=trust_coefficient, master_weights=True,
+                            zero_grad_in_step=True)
+    opt.max_grad_norm, opt.loss_scaling = _check_bound(max_grad_norm), bool(loss_scaling)
+    return opt
+
+
 class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
     def __init__(self, process_group, optimizer, average: bool = True):
         super().__init__(process_group, hierarchical=False, average=average)
@@ -549,7 +581,9 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         opt = self.optimizer
         is_adam = isinstance(opt, ShardedFusedAdam)
         is_lamb = isinstance(opt, ShardedFusedLamb)
-        if eng is None or bucket._slice is None or not (isinstance(opt, ShardedFusedSGD) or is_adam or is_lamb):
+        is_lars = isinstance(opt, ShardedFusedLars)
+        per_param = is_lamb or is_lars
+        if eng is None or bucket._slice is None or not (isinstance(opt, ShardedFusedSGD) or is_adam or per_param):
             return super().init_operations(bagua_ddp, bucket)
         bk = opt._bucketing
         group_index = getattr(bucket, "_fused_group", 0)
@@ -604,11 +638,11 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
                "state": (master, momentum, second) if is_adam or is_lamb else (master, momentum), "weights": wflat,
                "param_ids": [id(t) for t in bucket.tensors], "shard": None}
         bk.device = flat.device
-        if exchange or is_lamb:
+        if exchange or per_param:
             # phase A in the bucket program: reduce-scatter into the fp32 shard + per-CTA Σx² into this bucket's row of partials
             # (read by the norm exchange; nothing reads them without clipping); the update runs in step()
-            if is_lamb and bk.lamb is None:
-                bk.lamb = self._lamb_state(eng, bagua_ddp, bucket, flat.device)
+            if per_param and bk.lamb is None:
+                bk.lamb = self._per_param_state(eng, bagua_ddp, bucket, flat.device)
             if exchange and bk.clip is None:
                 bk.clip = self._clip_state(eng, bagua_ddp, bucket, flat.device, scaled)
             row = (bk.clip if exchange else bk.lamb)["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
@@ -617,8 +651,8 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
             bucket.backend_bucket.append_op(red)
             bucket._ops_keepalive.append(red)
             coef_ptr = bk.clip["out"][1:].data_ptr() if exchange else 0
-        if is_lamb:
-            op, moments = self._lamb_ops(eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr)
+        if per_param:
+            op, moments = self._per_param_ops(eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr, is_lars)
         elif exchange and is_adam:
             op = C.ShardAdamOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
                                second.data_ptr(), use_mc, cfg)
@@ -631,14 +665,14 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         else:
             op = C.AllReduceSgdOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                   master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
-        if exchange or is_lamb:
+        if exchange or per_param:
             bk.update_ops.append(op)
         else:
             bucket.backend_bucket.append_op(op)
         bucket._ops_keepalive.append(op)
-        kind = "fused_lamb_" if is_lamb else ("fused_adam_" if is_adam else "fused_sgd_")
+        kind = "fused_lamb_" if is_lamb else ("fused_lars_" if is_lars else ("fused_adam_" if is_adam else "fused_sgd_"))
         bucket.allreduce_variant = kind + ("scaled_" if scaled else "") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
-        rec["step_ops"] = (op, moments) if is_lamb else (op,)   # the update op first: state_dict() saves its count
+        rec["step_ops"] = (op, moments) if per_param else (op,)   # the update op first: state_dict() saves its count
         if scaled:   # the ops obey the exchange's vote and take the step count it keeps on the device
             for o in rec["step_ops"]:
                 o.set_device_step(coef_ptr, bk.clip["t"].data_ptr())
@@ -647,9 +681,10 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         opt._register_shard(rec)
         opt._sync_hyper()
 
-    def _lamb_state(self, eng, bagua_ddp, bucket, device):
-        """State of the LAMB ratio exchange, shared by all buckets: a global index of the bucketed parameters (bucket order,
-        padding excluded), the per-parameter outputs (fp32 ratio, fp64 {Σw², Σu²}), the stage-1 partial tables filled in bucket by
+    def _per_param_state(self, eng, bagua_ddp, bucket, device):
+        """State of the per-parameter exchange of LAMB and LARS (LambRatioOp), shared by all buckets: a global index of the bucketed
+        parameters (bucket order, padding excluded), the per-parameter outputs (fp32 LAMB ratio, unused by LARS; the global fp64
+        pairs, {Σw², Σu²} for LAMB and {Σw², Σg²} for LARS), the stage-1 partial tables filled in bucket by
         bucket, the phase-A partial sums when no norm exchange provides them, and the symmetric box (2 halves × MAX_PEERS ×
         parameters × 2 doubles, freed with the first bucket's other symmetric slices when the buckets are rebuilt)."""
         import torch
@@ -666,10 +701,11 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
                 "seg_ptr": [0] * len(names), "seg_nblk": [0] * len(names), "ratio_op": None,
                 "partials": torch.zeros(len(bagua_ddp.bagua_buckets), C.MAX_COMM_BLOCKS, dtype=torch.float64, device=device)}
 
-    def _lamb_ops(self, eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr):
-        """The LAMB ops of one bucket, after phase A: the moments op over the shard's segments (parameter ∩ [lo, hi), shard-local
-        offsets), whose per-block partials the ratio exchange sums per parameter, and the apply op. The ratio exchange is built once
-        every bucketed parameter has its table entry."""
+    def _per_param_ops(self, eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr, lars):
+        """The ops of one LAMB or LARS bucket, after phase A: the stage-1 op over the shard's segments (parameter ∩ [lo, hi),
+        shard-local offsets) — LAMB's moments over [master, shard, m1, m2], LARS's norms over [master, shard] — whose per-block
+        partials the exchange sums per parameter, and the apply op. The exchange is built once every bucketed parameter has its
+        table entry."""
         import torch
 
         from ...core import native
@@ -677,19 +713,20 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
 
         C = native()
         lam = bk.lamb
-        master, m1, m2 = rec["state"]
-        shard, lo, hi, dev = rec["shard"], rec["lo"], rec["hi"], bk.device
-        segs, views = [], [[], [], [], []]
+        master, shard, lo, hi, dev = rec["state"][0], rec["shard"], rec["lo"], rec["hi"], bk.device
+        lists = (master, shard) if lars else (master, shard) + tuple(rec["state"][1:])
+        Stage1 = C.LarsNormsOp if lars else C.LambMomentsOp
+        segs, views = [], [[] for _ in lists]
         for name, off, n, _, _ in rec["layout"]:
             a, b = max(off, lo), min(off + n, hi)
             if a < b:
                 segs.append((a - lo, b - lo, lam["index"][name]))
-                for lst, buf in zip(views, (master, shard, m1, m2)):
+                for lst, buf in zip(views, lists):
                     lst.append(buf[a - lo: b - lo])
         if segs:
             plan = multi_tensor_plan(views)
             partials = torch.zeros(max(plan.n_blocks, 1), 2, dtype=torch.float64, device=dev)
-            moments = C.LambMomentsOp(*plan.args(), coef_ptr, partials.data_ptr())
+            moments = Stage1(*plan.args(), coef_ptr, partials.data_ptr())
             blk = 0
             for a, b, t in segs:   # the plan gives each segment ceil(len / CHUNK) consecutive blocks, in segment order
                 nb = (b - a + plan.CHUNK - 1) // plan.CHUNK
@@ -698,10 +735,14 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
             assert blk == plan.n_blocks
         else:   # an empty slice (small bucket, many ranks): no moments to update, but the rank still takes part in every exchange
             plan, partials = None, torch.zeros(1, 2, dtype=torch.float64, device=dev)
-            moments = C.LambMomentsOp(0, 0, 0, 0, 0, 0, 65536, coef_ptr, partials.data_ptr())
+            moments = Stage1(0, 0, 0, 0, 0, 0, 65536, coef_ptr, partials.data_ptr())
         table = torch.tensor([v for s in segs for v in s] or [0, 0, 0], dtype=torch.int32, device=dev)
-        op = C.ShardLambOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, master.data_ptr(), m1.data_ptr(), m2.data_ptr(), table.data_ptr(), len(segs),
-                           lam["ratio"].data_ptr(), use_mc, cfg)
+        if lars:
+            op = C.ShardLarsOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), rec["state"][1].data_ptr(),
+                               table.data_ptr(), len(segs), lam["sums"].data_ptr(), use_mc, cfg)
+        else:
+            op = C.ShardLambOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, master.data_ptr(), rec["state"][1].data_ptr(), rec["state"][2].data_ptr(),
+                               table.data_ptr(), len(segs), lam["ratio"].data_ptr(), use_mc, cfg)
         rec["lamb_tables"] = (plan, partials, table, segs)
         bk.pre_ops.append(moments)
         lam["pending"] -= {name for name, *_ in rec["layout"]}
@@ -717,7 +758,7 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
 
 class FusedGradientAllReduceAlgorithm(Algorithm):
     """Gradient allreduce whose buckets also apply the optimizer update (see :func:`make_sharded_fused_sgd` /
-    :func:`make_sharded_fused_adam`)."""
+    :func:`make_sharded_fused_adam` / :func:`make_sharded_fused_lamb` / :func:`make_sharded_fused_lars`)."""
 
     def __init__(self, optimizer, average: bool = True):
         self.optimizer = optimizer

@@ -36,7 +36,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspa
 import bagua_b200 as bagua  # noqa: E402
 from bagua_b200.models import get_model  # noqa: E402
 from bagua_b200.parallel.algorithms import Algorithm, q_adam  # noqa: E402
-from bagua_b200.parallel.algorithms.gradient_allreduce import FusedGradientAllReduceAlgorithm, make_sharded_fused_sgd  # noqa: E402
+from bagua_b200.parallel.algorithms.gradient_allreduce import FusedGradientAllReduceAlgorithm, make_sharded_fused_lars, make_sharded_fused_sgd  # noqa: E402
 
 
 def parse():
@@ -67,7 +67,11 @@ def parse():
     p.add_argument("--algorithm", default="gradient_allreduce", help="gradient_allreduce, bytegrad, decentralized, low_precision_decentralized, qadam, async")
     p.add_argument("--async-sync-interval", type=int, default=500)
     p.add_argument("--async-warmup-steps", type=int, default=100)
-    p.add_argument("--fused-shard", action="store_true", help="SGD inside the bucket kernels (reduce-scatter → update → all-gather)")
+    p.add_argument("--fused-shard", action="store_true", help="SGD inside the bucket kernels (reduce-scatter → update → all-gather); with "
+                   "--optimizer lars the sharded LARS (reduce-scatter in the buckets, update in step())")
+    p.add_argument("--optimizer", default="sgd", choices=["sgd", "lars"], help="momentum SGD, or LARS for large global batches (BatchNorm "
+                   "and bias parameters get no weight decay and no layer adaptation)")
+    p.add_argument("--trust-coefficient", type=float, default=1e-3, help="LARS trust coefficient (eta)")
     p.add_argument("--fuse-optimizer", action="store_true", help="generic fused optimizer (bagua.contrib.fuse_optimizer)")
     p.add_argument("--synthetic", action="store_true")
     p.add_argument("--steps-per-epoch", type=int, default=100, help="synthetic data only")
@@ -156,6 +160,17 @@ def make_optimizer(args, model, lr, cuda, world):
     if args.algorithm == "qadam":
         opt = q_adam.QAdamOptimizer(model.parameters(), lr=lr * 1e-2, warmup_steps=100)
         return opt, q_adam.QAdamAlgorithm(opt)
+    if args.optimizer == "lars":
+        if args.algorithm != "gradient_allreduce":
+            raise SystemExit("--optimizer lars runs with --algorithm gradient_allreduce")
+        # the MLPerf recipe: parameters with ndim <= 1 (BatchNorm, biases) in a weight_decay = 0 group, i.e. plain momentum SGD
+        groups = [{"params": [p for p in model.parameters() if p.dim() > 1], "weight_decay": args.weight_decay},
+                  {"params": [p for p in model.parameters() if p.dim() <= 1], "weight_decay": 0.0}]
+        kw = dict(lr=lr, momentum=args.momentum, trust_coefficient=args.trust_coefficient)
+        if args.fused_shard and cuda:
+            opt = make_sharded_fused_lars(groups, **kw)
+            return opt, FusedGradientAllReduceAlgorithm(opt)
+        return bagua.ops.FusedLARS(groups, **kw), Algorithm.init(args.algorithm)
     if args.fused_shard and cuda and args.algorithm == "gradient_allreduce":
         opt = make_sharded_fused_sgd(model.parameters(), lr=lr, momentum=args.momentum, weight_decay=args.weight_decay)
         return opt, FusedGradientAllReduceAlgorithm(opt)

@@ -128,7 +128,18 @@ lapply = C.ShardLambOp(comm, b.buf, 0, NB, code, master.data_ptr(), mom.data_ptr
 lapply.set_hyper(1e-3, 0.9, 0.999, 1e-6, 0.01)
 # reads master and both moments (12B); writes master (4B) + weights (2B) per element
 timed("shard_lamb_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(lapply), n * 18)
-del shard, lpart
+# in-bucket LARS on the same bucket as ONE parameter: stage-1 norms over [master, shard], apply from the exchanged sums
+nplan = multi_tensor_plan([[master], [shard]])
+npart = torch.zeros(nplan.n_blocks, 2, dtype=torch.float64, device=dev)
+lnorms = C.LarsNormsOp(*nplan.args(), 0, npart.data_ptr())
+# reads master and shard (8B) per element
+timed("multi_tensor_lars_stage1_kernel<f32> 32M-element shard (in-bucket norms)", lambda: run(lnorms), n * 8)
+lsums.copy_(torch.tensor([[float(n), float(n)]], dtype=torch.float64))
+lars = C.ShardLarsOp(comm, b.buf, 0, NB, code, shard.data_ptr(), 0, master.data_ptr(), mom.data_ptr(), lsegs.data_ptr(), 1, lsums.data_ptr(), False, w.cfg(32))
+lars.set_hyper(1e-3, 0.9, 5e-4, 1e-3)
+# reads shard, master, momentum (12B); writes master, momentum (8B) + weights (2B) per element
+timed("shard_lars_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(lars), n * 22)
+del shard, lpart, npart
 
 # single-GPU kernels ------------------------------------------------------------------------------------------------------
 P = 138 * 1000 * 1000 // 8 * 8   # VGG16-sized arena
