@@ -251,9 +251,13 @@ PYBIND11_MODULE(_C, m) {
                  py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"),
                  py::arg("cfg")));
     py::class_<ShardGradOp, CommOp, std::shared_ptr<ShardGradOp>>(m, "ShardGradOp")
-        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool, LaunchCfg>(), py::arg("comm"),
+        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool, LaunchCfg, bool>(), py::arg("comm"),
              py::arg("grads"), py::arg("g_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("partials_ptr"), py::arg("scale"),
-             py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg"));
+             py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg"), py::arg("accumulate") = false)
+        .def("restart", &ShardGradOp::restart)
+        .def("resume", &ShardGradOp::resume)
+        .def("pending", &ShardGradOp::pending)
+        .def("accumulate", &ShardGradOp::accumulate);
     py::class_<GradNormOp, CommOp, std::shared_ptr<GradNormOp>>(m, "GradNormOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, uint64_t, int, uint64_t, uint64_t>(), py::arg("comm"), py::arg("box"), py::arg("box_off"),
              py::arg("partials_ptr"), py::arg("nslots"), py::arg("extra_ptr"), py::arg("out_ptr"))

@@ -93,9 +93,12 @@ void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerB
 // Global-norm clipping of the in-bucket optimizers (see shard_grad_kernel): phase A reduce-scatters a bucket into the fp32 gradient
 // `shard` of the owned slice (scaled) and leaves one fp64 Σx² per CTA in partials[block]; grad_norm sums partials[0..nslots) and
 // *extra (nullable), exchanges the per-rank sums through the symmetric `box` (2·kMaxPeers doubles at box_off) and writes
-// out = {total, coef}; phase B applies SGD / Adam to the shard scaled by *coef and all-gathers the weights.
+// out = {total, coef}; phase B applies SGD / Adam to the shard scaled by *coef and all-gathers the weights. With `accumulate` phase A
+// adds the scaled reduction into the shard (gradient accumulation) and Σx² is the accumulated shard's; preload_shard_grad_accum
+// loads that instantiation for one dtype / world / flavour.
 void launch_shard_grad(const PeerCtx& ctx, const PeerBuf& grads, size_t g_off, size_t bytes, int dtype, float* shard, double* partials, float scale,
-                       bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream);
+                       bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream, bool accumulate = false);
+void preload_shard_grad_accum(int dtype, int world, bool use_multimem);
 void launch_grad_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots, const double* extra, float max_norm,
                       uint32_t parity, float* out, cudaStream_t stream);
 //

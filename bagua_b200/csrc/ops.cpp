@@ -148,10 +148,21 @@ void AllReduceAdamOp::run(Bucket&, StreamHandle stream, int) {
     steps_++;
 }
 
+ShardGradOp::ShardGradOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, size_t g_off, size_t bytes, int dtype, uint64_t shard, uint64_t partials,
+                         float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg, bool accumulate)
+    : comm_(std::move(comm)), grads_(grads), g_off_(g_off), bytes_(bytes), dtype_(dtype), shard_(shard), partials_(partials), scale_(scale),
+      zero_grads_(zero_grads), use_mc_(use_multimem), cfg_(cfg), accumulate_(accumulate) {
+    if (accumulate_) {
+        DeviceGuard g(comm_->device());
+        preload_shard_grad_accum(dtype_, comm_->world(), use_mc_);
+    }
+}
+
 void ShardGradOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("shard_grad");
+    const bool add = accumulate_ && !fresh_.exchange(false, std::memory_order_acq_rel);
     launch_shard_grad(comm_->ctx(), grads_.buf, g_off_, bytes_, dtype_, reinterpret_cast<float*>(shard_), reinterpret_cast<double*>(partials_), scale_,
-                      zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
+                      zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream), add);
 }
 
 void GradNormOp::run(Bucket&, StreamHandle stream, int) {

@@ -257,14 +257,22 @@ private:
 
 // Global-norm clipping of the in-bucket optimizers (see shard_grad_kernel). Phase A, in the bucket program: reduce-scatter of the
 // gradients into the fp32 shard of the owned slice, per-CTA fp64 Σx² into `partials` (kMaxCommBlocks doubles), bucket cleared.
+// An `accumulate` op sums micro-batches in the shard: its first run after construction or restart() overwrites the shard (the
+// kernel of a non-accumulating op), every later run adds to it. run() is called by the comm worker or the inline-issue thread,
+// restart() / resume() by the Python thread, hence the atomic.
 class ShardGradOp final : public CommOp {
 public:
     ShardGradOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, size_t g_off, size_t bytes, int dtype, uint64_t shard, uint64_t partials, float scale,
-                bool zero_grads, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), grads_(grads), g_off_(g_off), bytes_(bytes), dtype_(dtype), shard_(shard), partials_(partials), scale_(scale),
-          zero_grads_(zero_grads), use_mc_(use_multimem), cfg_(cfg) {}
+                bool zero_grads, bool use_multimem, LaunchCfg cfg, bool accumulate = false);
     const char* kind() const override { return "shard_grad_sumsq"; }
     void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return !accumulate_; }  // overwrite, then add
+    void restart() { fresh_.store(true, std::memory_order_release); }
+    // the shard holds a sum the next run adds to (a re-bucketing carried it over)
+    void resume() { fresh_.store(false, std::memory_order_release); }
+    // whether the shard holds a sum that the next run adds to
+    bool pending() const { return accumulate_ && !fresh_.load(std::memory_order_acquire); }
+    bool accumulate() const { return accumulate_; }
 
 private:
     std::shared_ptr<PeerComm> comm_;
@@ -275,6 +283,8 @@ private:
     float scale_;
     bool zero_grads_, use_mc_;
     LaunchCfg cfg_;
+    const bool accumulate_;
+    std::atomic<bool> fresh_{true};
 };
 
 // The norm exchange: out = {total, coef} (fp32, device) from the `nslots` partials of this rank plus *extra (fp64, the parameters

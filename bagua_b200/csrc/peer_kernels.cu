@@ -369,8 +369,12 @@ __global__ void __launch_bounds__(512)
 //      every peer's norm box → barrier → Σ over slots 0 .. P-1 in rank order, so every rank computes the same bits → total, coef.
 //   B  shard_{sgd,adam}_kernel, per bucket: the update of the shard scaled by coef (read from device memory: the host never sees
 //      the norm) → all-gather of the weights → closing barrier, so no rank's trainer reads weights a peer is still writing.
+// With ACCUM (gradient accumulation over micro-batches) phase A adds into the shard instead of overwriting it:
+// s ← fl32(s_old + fl32(red·scale)), the product and the sum rounded separately (no FMA), and Σx² is taken over the new s. Every
+// launch of an op walks the same vectors with the same grid, so the partials of the last micro-batch are Σs² of the accumulated
+// shard and the norm exchange is unchanged. The old shard is loaded together with the peer loads of each unrolled iteration.
 // ---------------------------------------------------------------------------------------------------------
-template <typename T, int P, bool USE_MC>
+template <typename T, int P, bool USE_MC, bool ACCUM>
 __global__ void __launch_bounds__(512)
     shard_grad_kernel(PeerCtx ctx, PeerBuf grads, size_t g_off, size_t total_vecs, float* shard, double* partials, float scale, int zero_grads) {
     __shared__ double s_warp[512 / 32];
@@ -380,16 +384,62 @@ __global__ void __launch_bounds__(512)
     const Slicing sl(total_vecs, P);
     double ss = 0.0;
     if (ok) {
-        reduce_owned_slice<T, P, USE_MC, kReduceUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t, size_t j, float* g) {
-            float4* sp = reinterpret_cast<float4*>(shard + j * N);
+        if constexpr (ACCUM) {
+            // reduce_owned_slice's loads and sum, with the old shard loaded alongside (written out here: sharing them with
+            // reduce_owned_slice changes the SASS of the kernels built on it)
+            struct Raw {
+                uint4 red[USE_MC ? 1 : P];
+                float4 old[N / 4];
+            };
+            const size_t base = static_cast<size_t>(ctx.rank) * sl.vpr;
+            walk_owned_slice<kReduceUnroll<P, USE_MC>, Raw>(
+                sl, ctx.rank,
+                [&](Raw& raw, size_t v) {
+                    if constexpr (USE_MC) {
+                        raw.red[0] = multimem_ld_reduce_add<T>(grads.mc + g_off + v * 16);
+                    } else {
 #pragma unroll
-            for (int k = 0; k < N; ++k) {
-                g[k] *= scale;
-                ss += static_cast<double>(g[k]) * static_cast<double>(g[k]);
-            }
+                        for (int i = 0; i < P; ++i) raw.red[i] = ld_peer16(grads.ptr[(ctx.rank + i) % P] + g_off + v * 16);
+                    }
+                    const float4* sp = reinterpret_cast<const float4*>(shard + (v - base) * N);
 #pragma unroll
-            for (int q = 0; q < N / 4; ++q) sp[q] = make_float4(g[4 * q], g[4 * q + 1], g[4 * q + 2], g[4 * q + 3]);
-        });
+                    for (int q = 0; q < N / 4; ++q) raw.old[q] = sp[q];
+                },
+                [&](Raw& raw, size_t, size_t j) {
+                    float g[N];
+                    Vec16<T>::unpack(raw.red[0], g);
+#pragma unroll
+                    for (int i = 1; i < (USE_MC ? 1 : P); ++i) {
+                        float f[N];
+                        Vec16<T>::unpack(raw.red[i], f);
+#pragma unroll
+                        for (int k = 0; k < N; ++k) g[k] += f[k];
+                    }
+                    float4* sp = reinterpret_cast<float4*>(shard + j * N);
+#pragma unroll
+                    for (int q = 0; q < N / 4; ++q) {
+                        const float o[4] = {raw.old[q].x, raw.old[q].y, raw.old[q].z, raw.old[q].w};
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            float& s = g[4 * q + k];
+                            s = __fadd_rn(o[k], __fmul_rn(s, scale));
+                            ss += static_cast<double>(s) * static_cast<double>(s);
+                        }
+                        sp[q] = make_float4(g[4 * q], g[4 * q + 1], g[4 * q + 2], g[4 * q + 3]);
+                    }
+                });
+        } else {
+            reduce_owned_slice<T, P, USE_MC, kReduceUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t, size_t j, float* g) {
+                float4* sp = reinterpret_cast<float4*>(shard + j * N);
+#pragma unroll
+                for (int k = 0; k < N; ++k) {
+                    g[k] *= scale;
+                    ss += static_cast<double>(g[k]) * static_cast<double>(g[k]);
+                }
+#pragma unroll
+                for (int q = 0; q < N / 4; ++q) sp[q] = make_float4(g[4 * q], g[4 * q + 1], g[4 * q + 2], g[4 * q + 3]);
+            });
+        }
         ok = peer_barrier(ctx, e0 + 2);
     }
     // the CTA's Σx² in a fixed order: a shuffle tree per warp, then the warps in index order
@@ -1012,19 +1062,35 @@ void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerB
 }
 
 void launch_shard_grad(const PeerCtx& ctx, const PeerBuf& grads, size_t g_off, size_t bytes, int dtype, float* shard, double* partials, float scale,
-                       bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream) {
+                       bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream, bool accumulate) {
     const size_t vecs = peer_vecs("shard_grad", bytes, g_off, 0, nblocks);
     if (nthreads % 32 || nthreads > 512) throw std::runtime_error("bagua: shard_grad needs whole warps, at most 512 threads");
     if (vecs == 0) return;
     dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
             dispatch_mc(use_multimem, [&](auto mc) {
-                shard_grad_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
-                    ctx, grads, g_off, vecs, shard, partials, scale, zero_grads ? 1 : 0);
+                dispatch_flag(accumulate, [&](auto acc) {
+                    shard_grad_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(acc)::value><<<nblocks, nthreads, 0, stream>>>(
+                        ctx, grads, g_off, vecs, shard, partials, scale, zero_grads ? 1 : 0);
+                });
             });
         });
     });
     check_launch("shard_grad");
+}
+
+// An accumulating phase-A op first launches its ACCUM instantiation mid-training, possibly while a peer kernel spins (see
+// preload_gate_kernels): the op loads it when it is built.
+void preload_shard_grad_accum(int dtype, int world, bool use_multimem) {
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                cudaFuncAttributes a;
+                cudaFuncGetAttributes(&a, shard_grad_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, true>);
+            });
+        });
+    });
+    cudaGetLastError();
 }
 
 void launch_grad_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots, const double* extra, float max_norm,

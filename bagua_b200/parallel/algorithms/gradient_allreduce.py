@@ -103,6 +103,7 @@ class _Bucketing:
         self.uncovered = None  # the parameters outside the buckets, looked up once
         self.clip = None       # the norm exchange shared by all buckets (max_grad_norm and / or loss_scaling), see _clip_state
         self.lamb = None       # the per-parameter exchange shared by all buckets (LAMB and LARS), see _per_param_state
+        self.unit = None       # fp32 1.0 on the device: the coefficient of an accumulated update without a norm exchange
         # the program step() runs after the norm exchange, on the current stream of `device`: every bucket's pre-update op (LAMB
         # moments, LARS norms), the per-parameter exchange, every bucket's update op; empty when the updates run in the bucket kernels
         self.pre_ops = []
@@ -121,6 +122,7 @@ class _ShardedStateMixin:
     _kind = "sgd"
     max_grad_norm = None
     loss_scaling = False
+    accumulate_grads = False
 
     def __init__(self, *a, **k):
         super().__init__(*a, **k)
@@ -138,8 +140,9 @@ class _ShardedStateMixin:
     def native_ops_in_step(self) -> bool:
         """Whether ``step()`` runs native kernels once the bucket kernels are live: the norm exchange and the clipped update with
         ``max_grad_norm`` or ``loss_scaling``, LAMB's and LARS's per-bucket norms, per-parameter exchange and update always. They carry
-        per-call host state (box parity, step count), so such a step cannot be captured in a CUDA graph."""
-        return self.max_grad_norm is not None or self.loss_scaling or self._kind in _PER_PARAMETER
+        per-call host state (box parity, step count), so such a step cannot be captured in a CUDA graph. With ``accumulate_grads``
+        the update always runs in ``step()``, which also restarts the accumulated sum."""
+        return self.max_grad_norm is not None or self.loss_scaling or self._kind in _PER_PARAMETER or self.accumulate_grads
 
     def _gather(self, t, group):
         import torch
@@ -189,6 +192,36 @@ class _ShardedStateMixin:
             op.set_steps(int(sd.get("steps", 0)))
         if self.loss_scaling:
             self._bucketing.clip["t"].fill_(int(sd.get("steps", 0)))
+        if sd.get("grad_sum") is not None and rec.get("grad_op") is not None:   # a re-bucketing mid-accumulation: continue the sum
+            rec["shard"].copy_(shard_of(sd["grad_sum"], rec["layout"], rec["numel"], rec["lo"], rec["hi"], rec["shard"].numel(), device=rec["shard"].device))
+            rec["grad_op"].resume()
+
+    # ---- gradient accumulation (``accumulate_grads``) ----------------------------------------------------------------------
+    def _grad_sum(self):
+        """The pending accumulated gradient in consolidated form (``{name: fp32 tensor}``, like a state tensor), or ``None`` when no
+        micro-batch has been reduced since the last ``step()`` / ``zero_grad()``. Collective when a sum is pending; phase A is a
+        collective too, so every rank agrees on that."""
+        recs = [rec for rec in self._bucketing.shards if rec.get("grad_op") is not None]
+        if not any(rec["grad_op"].pending() for rec in recs):
+            return None
+        out = {}
+        for rec in recs:   # a bucket whose phase A has not run since the restart holds the last step's shard: it contributes zeros
+            t = rec["shard"] if rec["grad_op"].pending() else rec["shard"].new_zeros(rec["shard"].shape)
+            out.update(consolidate_shards(self._gather(t, rec["group"]), rec["numel"], rec["layout"]))
+        return out
+
+    def _restart_grad_sums(self):
+        """The next phase A of every bucket overwrites its shard: the accumulated gradient is consumed or discarded."""
+        for rec in self._bucketing.shards:
+            if rec.get("grad_op") is not None:
+                rec["grad_op"].restart()
+
+    def zero_grad(self, set_to_none: bool = False):
+        """Also discards the gradient accumulated in the shards (``accumulate_grads``), except right after ``step()``, which has
+        started a new sum already."""
+        if self.accumulate_grads and not self._grads_zeroed:
+            self._restart_grad_sums()
+        return super().zero_grad(set_to_none)
 
     def refresh_master_weights(self):
         """Re-read the fp32 master shards from the model weights (call after loading or editing weights without optimizer
@@ -271,6 +304,8 @@ class _ShardedStateMixin:
             total = super().clip_grad_norm_(max_norm, norm_type)
             self._norm_pending, self._last_norm = True, total
             return total
+        if self._bucketing.clip is None and self.accumulate_grads:
+            raise RuntimeError("this in-bucket optimizer has no norm exchange; construct it with max_grad_norm=... to clip the accumulated gradient")
         if self._bucketing.clip is None:
             raise RuntimeError("the in-bucket optimizer applied this step's update during backward, so its gradients cannot be clipped "
                                "afterwards; construct it with max_grad_norm=... (make_sharded_fused_sgd / make_sharded_fused_adam) to clip "
@@ -313,7 +348,8 @@ class _ShardedStateMixin:
         run the step program of the bucketing on the current stream (see :class:`_Bucketing`; empty when the bucket kernels of
         this iteration's backward already applied the update); then step the parameters outside the buckets, their gradients
         scaled by the exchange's coefficient. No host synchronisation, except with ``loss_scaling`` when the model has parameters
-        outside the buckets (see ``_step_uncovered``).
+        outside the buckets (see ``_step_uncovered``). With ``accumulate_grads`` the update consumes the gradient accumulated since the
+        last ``step()`` and the next backward starts a new sum, also when the step was skipped.
 
         With ``loss_scaling`` the exchange also unscales by the loss scale (``set_loss_scale``; 1 when ``step()`` is called
         without a scaler) and votes on overflow: a step whose averaged gradient holds an inf or a NaN changes no weight, no
@@ -350,6 +386,8 @@ class _ShardedStateMixin:
                 C.run_op(b.lamb["ratio_op"], stream, dev)
             for op in b.update_ops:
                 C.run_op(op, stream, dev)
+        if self.accumulate_grads:
+            self._restart_grad_sums()
         self._step_uncovered(coef, found_inf)
         self._grads_zeroed = True
         self.kernel_launches += b.launches
@@ -378,7 +416,8 @@ def _check_bound(max_grad_norm):
     return None if max_grad_norm is None else float(max_grad_norm)
 
 
-def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, max_grad_norm=None, loss_scaling=False):
+def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, max_grad_norm=None, loss_scaling=False,
+                           accumulate_grads=False):
     """SGD whose update runs *inside* each bucket's NVSwitch kernel (``allreduce_sgd_kernel``): reduce-scatter of the
     gradients → SGD(momentum) on this rank's 1/N shard with fp32 master weights → all-gather of the updated weights, one
     launch per bucket, overlapped with the rest of backward.  Optimizer state is sharded N ways (ZeRO-1-like) and the
@@ -393,7 +432,17 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
     ``loss_scaling``: dynamic loss scaling for fp16 training, driven by :class:`bagua_b200.amp.ShardedGradScaler`. The bucket
     program is the one of ``max_grad_norm`` (which stays optional: the norm it bounds and reports is the unscaled gradient's);
     the norm exchange also divides by the loss scale and decides, with the same bits on every rank, whether the step overflowed;
-    an overflowed step changes nothing anywhere and does not count (``last_step_skipped``)."""
+    an overflowed step changes nothing anywhere and does not count (``last_step_skipped``).
+
+    ``accumulate_grads``: gradient accumulation over micro-batches in the fp32 shard. Every backward pass that communicates adds
+    its averaged gradient into this rank's fp32 gradient shard (the bucket program is the one of ``max_grad_norm``, and the update
+    always runs in ``step()``, with a coefficient of exactly 1 when nothing clips or unscales); ``step()`` applies the update to
+    the sum, clipped and unscaled as a whole, and starts a new sum, also when loss scaling skips the step. ``zero_grad()`` between
+    two ``step()`` calls discards the sum. Micro-batches under ``no_sync()`` add up locally in the bucket and join the sum with the
+    next communicating backward. Needs ``FusedGradientAllReduceAlgorithm(average=True)``. Without a peer engine the bucket
+    all-reduce averages the locally accumulated bucket in place on each communicating backward, so the sum is kept in the
+    model's dtype there. Without the flag a second backward before ``step()`` overwrites the shard on the two-phase programs (and
+    SGD / Adam without clipping update the weights inside every backward): only the last micro-batch reaches the update."""
     from ...ops.optim import FusedSGD
 
     class _ShardedFusedSGD(_ShardedStateMixin, FusedSGD, ShardedFusedSGD):
@@ -401,7 +450,7 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
 
     opt = _ShardedFusedSGD(params, lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
                            master_weights=True, zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling = _check_bound(max_grad_norm), bool(loss_scaling)
+    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
     return opt
 
 
@@ -409,11 +458,12 @@ class ShardedFusedAdam(object):
     """Marker mix-in: see :func:`make_sharded_fused_adam`."""
 
 
-def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False, max_grad_norm=None, loss_scaling=False):
+def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False, max_grad_norm=None, loss_scaling=False,
+                            accumulate_grads=False):
     """Adam / AdamW counterpart of :func:`make_sharded_fused_sgd`: the update of this rank's 1/N shard (fp32 master weights
     and both moments) runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_adam_kernel``).  With one
     process (or without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedAdam`.  ``max_grad_norm``,
-    ``loss_scaling``: see :func:`make_sharded_fused_sgd`."""
+    ``loss_scaling``, ``accumulate_grads``: see :func:`make_sharded_fused_sgd`."""
     from ...ops.optim import FusedAdam
 
     class _ShardedFusedAdam(_ShardedStateMixin, FusedAdam, ShardedFusedAdam):
@@ -421,7 +471,7 @@ def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weigh
 
     opt = _ShardedFusedAdam(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, adamw=adamw, master_weights=True,
                             zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling = _check_bound(max_grad_norm), bool(loss_scaling)
+    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
     return opt
 
 
@@ -429,7 +479,8 @@ class ShardedFusedLamb(object):
     """Marker mix-in: see :func:`make_sharded_fused_lamb`."""
 
 
-def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01, max_grad_norm=None, loss_scaling=False):
+def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01, max_grad_norm=None, loss_scaling=False,
+                            accumulate_grads=False):
     """LAMB (apex ``FusedLAMB`` semantics, see :class:`bagua_b200.ops.optim.FusedLAMB`) on the in-bucket sharded path: each rank
     keeps fp32 master weights and both moments for its 1/N slice of every bucket.
 
@@ -441,14 +492,15 @@ def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weigh
     all-gather of the weights per bucket — ``2·buckets + 1`` launches (+1 with clipping). A parameter group with
     ``weight_decay=0`` gets no layer adaptation (ratio 1). With one process, or without a peer engine, it behaves like
     :class:`bagua_b200.ops.optim.FusedLAMB`; see ``docs/algorithms.md``. ``loss_scaling``: see :func:`make_sharded_fused_sgd`;
-    a skipped step also leaves the moments alone, and its ratio exchange runs with an unused result."""
+    a skipped step also leaves the moments alone, and its ratio exchange runs with an unused result. ``accumulate_grads``: see
+    :func:`make_sharded_fused_sgd`; the moments and the trust ratios see the accumulated gradient."""
     from ...ops.optim import FusedLAMB
 
     class _ShardedFusedLamb(_ShardedStateMixin, FusedLAMB, ShardedFusedLamb):
         _kind = "lamb"
 
     opt = _ShardedFusedLamb(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, master_weights=True, zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling = _check_bound(max_grad_norm), bool(loss_scaling)
+    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
     return opt
 
 
@@ -456,7 +508,8 @@ class ShardedFusedLars(object):
     """Marker mix-in: see :func:`make_sharded_fused_lars`."""
 
 
-def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, trust_coefficient=1e-3, max_grad_norm=None, loss_scaling=False):
+def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, trust_coefficient=1e-3, max_grad_norm=None, loss_scaling=False,
+                            accumulate_grads=False):
     """LARS (see :class:`bagua_b200.ops.optim.FusedLARS`) on the in-bucket sharded path: each rank keeps fp32 master weights and
     the momentum for its 1/N slice of every bucket.
 
@@ -467,7 +520,7 @@ def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, tru
     the momentum, the update and the all-gather of the weights per bucket — ``2·buckets + 1`` launches (+1 with the norm
     exchange). The gradient the norms and the update see is the clipped / unscaled one. Put parameters with ``ndim ≤ 1``
     (biases, BatchNorm) in a ``weight_decay=0`` group: they get plain momentum SGD. With one process, or without a peer engine, it
-    behaves like :class:`bagua_b200.ops.optim.FusedLARS`; ``loss_scaling``: see :func:`make_sharded_fused_sgd`."""
+    behaves like :class:`bagua_b200.ops.optim.FusedLARS`; ``loss_scaling``, ``accumulate_grads``: see :func:`make_sharded_fused_sgd`."""
     from ...ops.optim import FusedLARS
 
     class _ShardedFusedLars(_ShardedStateMixin, FusedLARS, ShardedFusedLars):
@@ -475,7 +528,7 @@ def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, tru
 
     opt = _ShardedFusedLars(params, lr=lr, momentum=momentum, weight_decay=weight_decay, trust_coefficient=trust_coefficient, master_weights=True,
                             zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling = _check_bound(max_grad_norm), bool(loss_scaling)
+    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
     return opt
 
 
@@ -509,12 +562,15 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         """Called at the start of every (re-)bucketing — with_bagua, the autotune service moving bucket boundaries every 100 steps,
         the find_unused_parameters rebuild: snapshot the sharded master weights / moments / step count in their consolidated
         (world-size and bucketing independent) form and forget the old bucketing; ``init_operations`` re-shards from the snapshot.
-        Collective (an all-gather per state tensor), like re-bucketing itself."""
+        Collective (an all-gather per state tensor), like re-bucketing itself. A gradient accumulated in the shards since the last
+        ``step()`` (``accumulate_grads``) is carried over the same way, and the new phase-A ops add to it."""
         opt = self.optimizer
         if not isinstance(opt, _ShardedStateMixin):
             return
         if opt._bucketing.shards:
             opt._pending_state = opt.state_dict()
+            if opt.accumulate_grads:
+                opt._pending_state["grad_sum"] = opt._grad_sum()
         opt._bucketing = _Bucketing()
 
     def tensors_to_buckets(self, tensors, do_flatten):
@@ -630,33 +686,40 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         scale = (1.0 / n) if self.average else 1.0
         code = dtype_code(flat.dtype)
         second = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device) if is_adam or is_lamb else None
-        clip, scaled = opt.max_grad_norm is not None, opt.loss_scaling
+        clip, scaled, accum = opt.max_grad_norm is not None, opt.loss_scaling, opt.accumulate_grads
         exchange = clip or scaled   # the norm exchange runs in step(), so the update does too
+        two_phase = exchange or per_param or accum
         layout = [(t.bagua_tensor_name, (t.bagua_getter_closure().data_ptr() - base) // flat.element_size(), t.bagua_getter_closure().numel(),
                    tuple(t.shape), tuple(dense_strides(t))) for t in bucket.tensors if not t.bagua_tensor_name.startswith("bagua_padding_tensor")]
         rec = {"bucket": bucket.name, "group": self.process_group, "numel": flat.numel(), "lo": lo, "hi": hi, "layout": layout,
                "state": (master, momentum, second) if is_adam or is_lamb else (master, momentum), "weights": wflat,
                "param_ids": [id(t) for t in bucket.tensors], "shard": None}
         bk.device = flat.device
-        if exchange or per_param:
-            # phase A in the bucket program: reduce-scatter into the fp32 shard + per-CTA Σx² into this bucket's row of partials
-            # (read by the norm exchange; nothing reads them without clipping); the update runs in step()
+        if two_phase:
+            # phase A in the bucket program: reduce-scatter into the fp32 shard (added to it when accumulating) + per-CTA Σx² into
+            # this bucket's row of partials (read by the norm exchange; nothing reads them without clipping); the update runs in step()
             if per_param and bk.lamb is None:
                 bk.lamb = self._per_param_state(eng, bagua_ddp, bucket, flat.device)
             if exchange and bk.clip is None:
                 bk.clip = self._clip_state(eng, bagua_ddp, bucket, flat.device, scaled)
-            row = (bk.clip if exchange else bk.lamb)["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
+            if exchange or per_param:
+                row = (bk.clip if exchange else bk.lamb)["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
+            else:   # SGD / Adam accumulating without a norm exchange: partials nobody reads, and an update coefficient of exactly 1
+                row = rec["partials"] = torch.zeros(C.MAX_COMM_BLOCKS, dtype=torch.float64, device=flat.device)
+                if bk.unit is None:
+                    bk.unit = torch.ones(1, dtype=torch.float32, device=flat.device)
             shard = rec["shard"] = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
-            red = C.ShardGradOp(eng.comm, bucket._slice.buf, bucket._slice.offset, nbytes, code, shard.data_ptr(), row.data_ptr(), scale, True, use_mc, cfg)
+            args = (eng.comm, bucket._slice.buf, bucket._slice.offset, nbytes, code, shard.data_ptr(), row.data_ptr(), scale, True, use_mc, cfg)
+            red = rec["grad_op"] = C.ShardGradOp(*args, True) if accum else C.ShardGradOp(*args)
             bucket.backend_bucket.append_op(red)
             bucket._ops_keepalive.append(red)
-            coef_ptr = bk.clip["out"][1:].data_ptr() if exchange else 0
+            coef_ptr = bk.clip["out"][1:].data_ptr() if exchange else (bk.unit.data_ptr() if not per_param else 0)
         if per_param:
             op, moments = self._per_param_ops(eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr, is_lars)
-        elif exchange and is_adam:
+        elif two_phase and is_adam:
             op = C.ShardAdamOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
                                second.data_ptr(), use_mc, cfg)
-        elif exchange:
+        elif two_phase:
             op = C.ShardSgdOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
                               use_mc, cfg)
         elif is_adam:
@@ -665,13 +728,13 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         else:
             op = C.AllReduceSgdOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                   master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
-        if exchange or per_param:
+        if two_phase:
             bk.update_ops.append(op)
         else:
             bucket.backend_bucket.append_op(op)
         bucket._ops_keepalive.append(op)
         kind = "fused_lamb_" if is_lamb else ("fused_lars_" if is_lars else ("fused_adam_" if is_adam else "fused_sgd_"))
-        bucket.allreduce_variant = kind + ("scaled_" if scaled else "") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
+        bucket.allreduce_variant = kind + ("accum_" if accum else "") + ("scaled_" if scaled else "") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
         rec["step_ops"] = (op, moments) if per_param else (op,)   # the update op first: state_dict() saves its count
         if scaled:   # the ops obey the exchange's vote and take the step count it keeps on the device
             for o in rec["step_ops"]:
@@ -765,5 +828,9 @@ class FusedGradientAllReduceAlgorithm(Algorithm):
         self.average = average
 
     def reify(self, process_group):
+        # On the fallback path the bucket all-reduce runs in place on an already accumulated bucket: right only when it averages.
+        if getattr(self.optimizer, "accumulate_grads", False) and not self.average:
+            raise ValueError("accumulate_grads=True needs FusedGradientAllReduceAlgorithm(average=True): the accumulated gradient is the sum of the "
+                             "micro-batches' averaged gradients")
         # optimizer state is carried across (re-)bucketing by the impl (tensors_to_buckets → _carry_state_over)
         return FusedGradientAllReduceAlgorithmImpl(process_group, self.optimizer, average=self.average)

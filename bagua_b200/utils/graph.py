@@ -61,7 +61,7 @@ class GraphedTrainStep:
         for opt in self.optimizers:
             if getattr(opt, "native_ops_in_step", False):
                 raise NotImplementedError(f"{type(opt).__name__} runs native kernels from step() with per-call host state (box parity, "
-                                          "step count); it cannot be captured in a CUDA graph")
+                                          "step count, the restart of an accumulated gradient); it cannot be captured in a CUDA graph")
             why = graph_safe_optimizer(opt)
             if why is not None:
                 raise ValueError(f"optimizer cannot be captured in a CUDA graph: {why}")

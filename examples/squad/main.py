@@ -18,7 +18,9 @@ What each part is here (nothing is imported from ``transformers``; there is no n
   Without ``--train_file`` / ``--predict_file`` a template-generated SQuAD-format dataset stands in (``--num-synthetic`` paragraphs).
   Features are cached in ``--cache_dir`` (default: next to the data file) like the reference's ``cached_{train,dev}_…`` files.
 * optimisation — AdamW (decay on matrices only) with linear warm-up / decay, gradient clipping, gradient accumulation through
-  ``model.bagua_ddp.require_backward_grad_sync`` (micro-steps accumulate locally, the last one communicates).  On GPUs parameters are
+  ``model.bagua_ddp.require_backward_grad_sync`` (micro-steps accumulate locally, the last one communicates), or with
+  ``--fused-shard --accumulate-in-shard`` in the fp32 gradient shard of the in-bucket optimizer (every micro-step communicates and
+  adds its averaged gradient; ``accumulate_grads=True``).  On GPUs parameters are
   bf16 with fp32 master weights inside ``bagua_b200.ops.FusedAdam`` (``--fp16`` is accepted and means this mixed-precision path;
   ``--dtype fp32`` restores full precision; ``--dtype fp16`` trains in real fp16 with dynamic loss scaling, which needs
   ``--fused-shard``: ``ShardedGradScaler`` unscales, detects overflow and skips steps on the device); ``--fused-shard`` moves AdamW
@@ -111,6 +113,8 @@ def parse():
     a("--async-warmup-steps", type=int, default=100)
     a("--fuse-optimizer", action="store_true")
     a("--fused-shard", action="store_true", help="AdamW inside the bucket kernels (reduce-scatter → update → all-gather)")
+    a("--accumulate-in-shard", action="store_true",
+      help="with --fused-shard and --gradient_accumulation_steps > 1: every micro-step communicates and adds its gradient to the fp32 shard")
     a("--load-balance", action="store_true", help="LoadBalancingDistributedSampler keyed on the number of non-pad tokens")
     a("--dtype", default="bf16", choices=["bf16", "fp32", "fp16"], help="fp16: real fp16 with dynamic loss scaling, needs --fused-shard")
     a("--tiny", action="store_true", help="2-layer model (smoke tests)")
@@ -252,10 +256,12 @@ def make_optimizer(args, model, cuda, world):
     if args.algorithm == "qadam":
         opt = q_adam.QAdamOptimizer(model.parameters(), lr=args.learning_rate, warmup_steps=100, eps=args.adam_epsilon, weight_decay=args.weight_decay)
         return opt, q_adam.QAdamAlgorithm(opt)
-    if args.fused_shard and cuda and args.algorithm == "gradient_allreduce":
+    in_shard = args.accumulate_in_shard and args.gradient_accumulation_steps > 1
+    # without a GPU the in-shard accumulation runs on the fallback (all-reduce + flat AdamW), which accumulates in the model's dtype
+    if args.fused_shard and (cuda or in_shard) and args.algorithm == "gradient_allreduce":
         opt = make_sharded_fused_adam(groups, lr=args.learning_rate, eps=args.adam_epsilon, adamw=True,   # buckets are cut per parameter group
                                       max_grad_norm=args.max_grad_norm if args.max_grad_norm > 0 else None,   # clipped inside step()
-                                      loss_scaling=args.dtype == "fp16")
+                                      loss_scaling=args.dtype == "fp16", accumulate_grads=in_shard)
         return opt, FusedGradientAllReduceAlgorithm(opt)
     if cuda and not args.fuse_optimizer:
         opt = bagua.ops.FusedAdam(groups, lr=args.learning_rate, eps=args.adam_epsilon, adamw=True)
@@ -316,6 +322,7 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
         return torch.cuda.nvtx.range(name) if (cuda and args.prof >= 0) else contextlib.nullcontext()
 
     sharded = isinstance(optimizer, ShardedFusedAdam)
+    in_shard = sharded and optimizer.accumulate_grads   # every micro-step communicates; step() consumes the sum in the shard
     grad_norm = None
     # fp16: the scaler hands its device scale to the sharded optimizer, whose step program unscales, votes on overflow and skips
     scaler = bagua.amp.ShardedGradScaler() if args.dtype == "fp16" else None
@@ -332,7 +339,7 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
                 torch.cuda.cudart().cudaProfilerStart()
             ids, tt, am, sp, ep = (x.to(dev, non_blocking=True) for x in batch)
             last_micro = (it + 1) % accum == 0
-            model.bagua_ddp.require_backward_grad_sync = last_micro     # earlier micro-steps accumulate locally
+            model.bagua_ddp.require_backward_grad_sync = last_micro or in_shard     # otherwise earlier micro-steps accumulate locally
             with nvtx(f"iteration {seen_iters}"):
                 with nvtx("forward"):
                     loss = model(ids, token_type_ids=tt, attention_mask=am, start_positions=sp, end_positions=ep)[0] / accum

@@ -139,7 +139,13 @@ lars = C.ShardLarsOp(comm, b.buf, 0, NB, code, shard.data_ptr(), 0, master.data_
 lars.set_hyper(1e-3, 0.9, 5e-4, 1e-3)
 # reads shard, master, momentum (12B); writes master, momentum (8B) + weights (2B) per element
 timed("shard_lars_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(lars), n * 22)
-del shard, lpart, npart
+# phase A into the same shard: overwrite (reads the bucket 2B, writes the shard 4B) and accumulate (+ reads the shard 4B) per element
+gpart = torch.zeros(C.MAX_COMM_BLOCKS, dtype=torch.float64, device=dev)
+for acc, nb in ((False, 6), (True, 10)):
+    sg = C.ShardGradOp(comm, a.buf, 0, NB, code, shard.data_ptr(), gpart.data_ptr(), 1.0, True, False, w.cfg(64), acc)
+    run(sg)   # an accumulating op overwrites on its first run
+    timed(f"shard_grad_kernel<bf16,P=1,peer,ACCUM={str(acc).lower()}> 64MiB bucket", lambda sg=sg: run(sg), n * nb)
+del shard, lpart, npart, gpart
 
 # single-GPU kernels ------------------------------------------------------------------------------------------------------
 P = 138 * 1000 * 1000 // 8 * 8   # VGG16-sized arena
