@@ -304,6 +304,14 @@ PYBIND11_MODULE(_C, m) {
                  py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
                  py::arg("master_ptr"), py::arg("momentum_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("sums_ptr"), py::arg("use_multimem"),
                  py::arg("cfg")));
+    py::class_<EmaOp, CommOp, std::shared_ptr<EmaOp>>(m, "EmaOp")
+        .def(py::init<uint64_t, uint64_t, uint64_t, uint64_t, int, int, int, float, uint64_t>(), py::arg("ptrs"), py::arg("sizes"), py::arg("b2t"),
+             py::arg("b2c"), py::arg("n_tensors"), py::arg("n_blocks"), py::arg("chunk"), py::arg("weight"), py::arg("vote_ptr"))
+        .def("set_weight", &EmaOp::set_weight)
+        .def("weight", &EmaOp::weight);
+    py::class_<ShardPublishOp, CommOp, std::shared_ptr<ShardPublishOp>>(m, "ShardPublishOp")
+        .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, bool, LaunchCfg>(), py::arg("comm"), py::arg("weights"),
+             py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("src_ptr"), py::arg("use_multimem"), py::arg("cfg"));
     py::class_<PeerAverageOp, CommOp, std::shared_ptr<PeerAverageOp>>(m, "PeerAverageOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, uint64_t, size_t, int, LaunchCfg>(), py::arg("comm"), py::arg("weights"),
              py::arg("off"), py::arg("out_ptr"), py::arg("bytes"), py::arg("dtype"), py::arg("cfg"))

@@ -135,6 +135,12 @@ void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off,
 void launch_shard_lars(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
                        float* master, float* momentum, const int32_t* segs, int nsegs, const double* sums, const LarsParams& hp, bool use_multimem,
                        int nblocks, int nthreads, cudaStream_t stream, bool vote = false);
+// Weight EMA of the in-bucket optimizers: publishes the fp32 shard `src` (the owned slice, shard-local like the master) rounded with
+// Vec16<T>::pack into every rank's copy of the weights, between an opening and a closing barrier. preload_shard_publish loads the
+// instantiation for one dtype / world / flavour.
+void launch_shard_publish(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* src, bool use_multimem,
+                          int nblocks, int nthreads, cudaStream_t stream);
+void preload_shard_publish(int dtype, int world, bool use_multimem);
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,
                          int nblocks, int nthreads, cudaStream_t stream);
 void launch_peer_barrier(const PeerCtx& ctx, cudaStream_t stream);
@@ -275,6 +281,9 @@ void launch_multi_tensor_lamb_stage2(const TensorListDesc& d, int dtype, bool mi
 void launch_multi_tensor_lars_stage1(const TensorListDesc& d, int dtype, bool mixed, const float* coef, double* sums, cudaStream_t stream, bool vote = false);
 void launch_multi_tensor_lars_stage2(const TensorListDesc& d, int dtype, bool mixed, const LarsParams& hp, const float* coef, const double* sums, bool zero_grad,
                                      cudaStream_t stream);
+// Exponential moving average of fp32 weights, lists [source(f32), ema(f32)]: e ← fl(e + fl(w·fl(m − e))), three separately rounded
+// operations. `vote` (nullable): with *vote != 0 (an overflowed loss-scaled step) nothing is written.
+void launch_multi_tensor_ema(const TensorListDesc& d, float weight, const float* vote, cudaStream_t stream);
 // QAdam momentum pre-step (bagua/torch_api/algorithms/q_adam.py:193-221): m = beta1*m + (1-beta1)*g
 void launch_qadam_momentum(float* exp_avg, const void* grad, int grad_dtype, size_t numel, float beta1, cudaStream_t stream);
 

@@ -571,6 +571,47 @@ void launch_multi_tensor_lars_stage2(const TensorListDesc& d, int dtype, bool mi
     check_launch("multi_tensor_lars_stage2");
 }
 
+// ---- exponential moving average of fp32 weights ---------------------------------------------------------------------
+// lists = [source(f32), ema(f32)]: e ← e + w·(m − e) with three separately rounded operations (the intrinsics keep the compiler from
+// contracting the product and the sum into an FMA), so a host fp32 emulation reproduces every bit. This is torch's lerp for w < 0.5.
+// A chunk takes 16-byte accesses when both of its pointers are 16-byte aligned (chunk offsets are multiples of 65536 elements, so
+// that is a property of the tensors' base addresses) and scalar ones otherwise: the lists may hold arbitrary views. `vote`
+// (nullable) is the loss-scaled step's found_inf word: when it is set the kernel writes nothing.
+__device__ __forceinline__ float ema_step(float e, float m, float w) { return __fadd_rn(e, __fmul_rn(w, __fsub_rn(m, e))); }
+
+__global__ void __launch_bounds__(kThreads) multi_tensor_ema_kernel(TensorListDesc d, float w, const float* vote) {
+    if (vote != nullptr && *vote != 0.f) return;
+    const int t = d.block_to_tensor[blockIdx.x];
+    const size_t off = static_cast<size_t>(d.block_to_chunk[blockIdx.x]) * d.chunk;
+    const size_t n = static_cast<size_t>(d.sizes[t]);
+    const size_t len = (n - off) < static_cast<size_t>(d.chunk) ? (n - off) : static_cast<size_t>(d.chunk);
+    const float* src = reinterpret_cast<const float*>(d.ptrs[t]) + off;
+    float* ema = reinterpret_cast<float*>(d.ptrs[d.n_tensors + t]) + off;
+    size_t done = 0;
+    if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(ema)) & 15u) == 0) {
+        const size_t nv = len / 4;
+        const float4* s4 = reinterpret_cast<const float4*>(src);
+        float4* e4 = reinterpret_cast<float4*>(ema);
+        for (size_t i = threadIdx.x; i < nv; i += blockDim.x) {
+            const float4 m = s4[i];
+            float4 e = e4[i];
+            e.x = ema_step(e.x, m.x, w);
+            e.y = ema_step(e.y, m.y, w);
+            e.z = ema_step(e.z, m.z, w);
+            e.w = ema_step(e.w, m.w, w);
+            e4[i] = e;
+        }
+        done = nv * 4;
+    }
+    for (size_t i = done + threadIdx.x; i < len; i += blockDim.x) ema[i] = ema_step(ema[i], src[i], w);
+}
+
+void launch_multi_tensor_ema(const TensorListDesc& d, float weight, const float* vote, cudaStream_t stream) {
+    if (d.n_blocks <= 0) return;
+    multi_tensor_ema_kernel<<<d.n_blocks, kThreads, 0, stream>>>(d, weight, vote);
+    check_launch("multi_tensor_ema");
+}
+
 // ---- QAdam momentum pre-step -------------------------------------------------------------------------------------
 template <typename GT>
 __global__ void __launch_bounds__(kThreads) qadam_momentum_kernel(float* __restrict__ m, const GT* __restrict__ g, size_t n, float beta1) {

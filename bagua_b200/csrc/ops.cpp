@@ -229,6 +229,21 @@ void ShardLarsOp::run(Bucket&, StreamHandle stream, int) {
     steps_++;
 }
 
+void EmaOp::run(Bucket&, StreamHandle stream, int) { launch_multi_tensor_ema(desc_, weight(), reinterpret_cast<const float*>(vote_), S(stream)); }
+
+ShardPublishOp::ShardPublishOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t src, bool use_multimem,
+                               LaunchCfg cfg)
+    : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), src_(src), use_mc_(use_multimem), cfg_(cfg) {
+    DeviceGuard g(comm_->device());
+    preload_shard_publish(dtype_, comm_->world(), use_mc_);
+}
+
+void ShardPublishOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("shard_publish");
+    launch_shard_publish(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(src_), use_mc_, cfg_.nblocks, cfg_.nthreads,
+                         S(stream));
+}
+
 int PeerAverageOp::shift_one_peer(int rank, int nranks, int64_t step) {
     const int64_t r = rank, n = nranks;
     if (rank < nranks / 2) return static_cast<int>(((step + r) % ((n + 1) / 2)) + (n / 2));

@@ -478,6 +478,44 @@ private:
     LaunchCfg cfg_;
 };
 
+// Weight EMA of the in-bucket optimizers. EmaOp is local: one multi-tensor launch of e ← e + w·(m − e) over the table's
+// [source, ema] pairs (every bucket's master and EMA shards, or the parameters outside the buckets), skipped on the device when the
+// vote word (nullable: the loss-scaled step's found_inf) is set. ShardPublishOp all-gathers an fp32 shard, rounded to the bucket's
+// dtype, into every rank's weights (see shard_publish_kernel).
+class EmaOp final : public CommOp {
+public:
+    EmaOp(uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, float weight, uint64_t vote)
+        : desc_{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes), reinterpret_cast<const int32_t*>(b2t),
+                reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk},
+          weight_(weight), vote_(vote) {}
+    const char* kind() const override { return "ema"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+    bool step_invariant() const override { return false; }  // the weight is the host's at launch
+    void set_weight(float w) { weight_.store(w, std::memory_order_relaxed); }
+    float weight() const { return weight_.load(std::memory_order_relaxed); }
+
+private:
+    TensorListDesc desc_;
+    std::atomic<float> weight_;
+    uint64_t vote_;
+};
+
+class ShardPublishOp final : public CommOp {
+public:
+    ShardPublishOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t src, bool use_multimem, LaunchCfg cfg);
+    const char* kind() const override { return "shard_publish"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf weights_;
+    size_t w_off_, bytes_;
+    int dtype_;
+    uint64_t src_;
+    bool use_mc_;
+    LaunchCfg cfg_;
+};
+
 // Decentralized SGD, shift_one pairing (peer formula: comm_ops/decentralized_full_precision_synchronous.rs:81-85).
 class PeerAverageOp final : public CommOp {
 public:

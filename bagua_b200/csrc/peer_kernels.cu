@@ -763,6 +763,25 @@ __global__ void __launch_bounds__(512) shard_lars_kernel(PeerCtx ctx, PeerBuf we
     store_epoch(ctx, e0 + 1);
 }
 
+// Publication of an fp32 shard as the bucket's weights: the walk of the update kernels with a copy in place of the update, so
+// Vec16<T>::pack(src) lands in every rank's copy of the owned slice. The weight EMA swaps its shard in with it and the master back
+// out; every update kernel publishes pack(master), so publishing the master restores the live weights bit for bit. Unlike an
+// update, which runs where the peers have passed the gradient exchange, this can follow any work of the trainer (an evaluation
+// pass on one rank while another has finished its own): the opening barrier waits until no rank still reads the weights.
+template <typename T, int P, bool USE_MC>
+__global__ void __launch_bounds__(512) shard_publish_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* src) {
+    const uint32_t e0 = load_epoch(ctx);
+    const bool ok = peer_barrier(ctx, e0 + 1);
+    if (ok) {
+        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), src, [](size_t, const float* s, float* w) {
+#pragma unroll
+            for (int k = 0; k < Vec16<T>::N; ++k) w[k] = s[k];
+        });
+        peer_barrier(ctx, e0 + 2);
+    }
+    store_epoch(ctx, e0 + 2);
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Decentralized SGD, shift_one: out = (mine + peer's weights) / 2, the peer's bucket being read straight over
 // NVLink (replaces grouped send/recv + average kernel, comm_ops/decentralized_full_precision_synchronous.rs:81-92).
@@ -1189,6 +1208,34 @@ void launch_shard_lars(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off,
         });
     });
     check_launch("shard_lars");
+}
+
+void launch_shard_publish(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* src, bool use_multimem,
+                          int nblocks, int nthreads, cudaStream_t stream) {
+    const size_t vecs = peer_vecs("shard_publish", bytes, w_off, 0, nblocks);
+    if (vecs == 0) return;
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(ctx.world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                shard_publish_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(ctx, weights, w_off, vecs,
+                                                                                                                              src);
+            });
+        });
+    });
+    check_launch("shard_publish");
+}
+
+// Loaded when the op is built, like the accumulating phase-A kernel: its first launch comes mid-training.
+void preload_shard_publish(int dtype, int world, bool use_multimem) {
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                cudaFuncAttributes a;
+                cudaFuncGetAttributes(&a, shard_publish_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value>);
+            });
+        });
+    });
+    cudaGetLastError();
 }
 
 void launch_peer_average(const PeerCtx& ctx, const PeerBuf& weights, size_t off, int peer, void* out, size_t bytes, int dtype,

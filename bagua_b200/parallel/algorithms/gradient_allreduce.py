@@ -5,6 +5,8 @@ the 1/N average; ``fused_optimizer=True`` additionally folds the SGD update of t
 of the updated weights into that kernel (see ``FusedShardedSGD``)."""
 from __future__ import annotations
 
+import contextlib
+
 from .base import Algorithm, AlgorithmImpl
 
 __all__ = ["GradientAllReduceAlgorithm", "GradientAllReduceAlgorithmImpl"]
@@ -110,6 +112,7 @@ class _Bucketing:
         self.update_ops = []
         self.device = None
         self.launches = 0      # optimizer-update kernels per step, in the bucket programs or in step()
+        self.ema = None        # ema_decay: the EmaOp over every bucket's [master, EMA] shard pair and its table, built with the last bucket
 
 
 class _ShardedStateMixin:
@@ -123,6 +126,9 @@ class _ShardedStateMixin:
     max_grad_norm = None
     loss_scaling = False
     accumulate_grads = False
+    ema_decay = None
+    ema_every = 1
+    _ema = False                     # built with ema_decay: an fp32 EMA next to every master
 
     def __init__(self, *a, **k):
         super().__init__(*a, **k)
@@ -131,6 +137,13 @@ class _ShardedStateMixin:
         self._norm_pending = False   # clip_grad_norm_ has computed this step's norm
         self._last_norm = None
         self._loss_scale = None      # the device tensor the norm exchange reads the loss scale from (None: a constant 1)
+        self._ema_calls = 0          # step() calls so far: the EMA updates on every ema_every-th
+        self._ema_swapped = False    # inside ema_weights()
+        self._ema_plans = {}         # tables (and EmaOps) of the local EMA launches, by role
+        self._param_names = {}       # id(parameter) → its name in the model, for ema_state_dict()
+
+    def _state_keys(self):
+        return _STATE_KEYS[self._kind] + (("ema",) if self._ema else ())
 
     @property
     def collective_state_dict(self) -> bool:
@@ -141,8 +154,9 @@ class _ShardedStateMixin:
         """Whether ``step()`` runs native kernels once the bucket kernels are live: the norm exchange and the clipped update with
         ``max_grad_norm`` or ``loss_scaling``, LAMB's and LARS's per-bucket norms, per-parameter exchange and update always. They carry
         per-call host state (box parity, step count), so such a step cannot be captured in a CUDA graph. With ``accumulate_grads``
-        the update always runs in ``step()``, which also restarts the accumulated sum."""
-        return self.max_grad_norm is not None or self.loss_scaling or self._kind in _PER_PARAMETER or self.accumulate_grads
+        the update always runs in ``step()``, which also restarts the accumulated sum; with ``ema_decay`` ``step()`` runs the EMA
+        update on every ``ema_every``-th call."""
+        return self.max_grad_norm is not None or self.loss_scaling or self._kind in _PER_PARAMETER or self.accumulate_grads or self._ema
 
     def _gather(self, t, group):
         import torch
@@ -154,11 +168,14 @@ class _ShardedStateMixin:
 
     def state_dict(self):
         if not self._bucketing.shards:
-            return super().state_dict()
+            sd = super().state_dict()
+            if self._ema:
+                sd["ema_calls"] = self._ema_calls
+            return sd
         state = {}
         steps = 0
         for rec in self._bucketing.shards:
-            for key, t in zip(_STATE_KEYS[self._kind], rec["state"]):
+            for key, t in zip(self._state_keys(), rec["state"]):
                 for name, full in consolidate_shards(self._gather(t, rec["group"]), rec["numel"], rec["layout"]).items():
                     state.setdefault(name, {})[key] = full.cpu()
             steps = max(steps, int(rec["step_ops"][0].steps()))
@@ -166,15 +183,31 @@ class _ShardedStateMixin:
             steps = int(self._bucketing.clip["t"].item())
         groups = [{k: v for k, v in g.items() if k != "params"} for g in self.param_groups]
         # parameters outside the buckets (MoE experts, ignored ones) are stepped by the base class: their state in torch's format
-        return {"sharded_fused": self._kind, "steps": steps, "state": state, "param_groups": groups, "uncovered": super().state_dict()}
+        out = {"sharded_fused": self._kind, "steps": steps, "state": state, "param_groups": groups, "uncovered": super().state_dict()}
+        if self._ema:
+            out["ema_calls"] = self._ema_calls
+        return out
+
+    def _load_local_ema(self, sd):
+        """The local EMAs (fallback path, parameters outside the buckets) travel as ``state[p]["ema"]`` in torch's format: dropped
+        when this optimizer keeps none; when the checkpoint has none they start from the loaded master at their next use."""
+        if not self._ema:
+            for st in self.state.values():
+                if isinstance(st, dict):
+                    st.pop("ema", None)
+        elif isinstance(sd, dict):
+            self._ema_calls = int(sd.get("ema_calls", 0))
 
     def load_state_dict(self, sd):
         if not isinstance(sd, dict) or "sharded_fused" not in sd:
-            return super().load_state_dict(sd)
+            out = super().load_state_dict(sd)
+            self._load_local_ema(sd)
+            return out
         if sd["sharded_fused"] != self._kind:
             raise ValueError(f"checkpoint holds {sd['sharded_fused']} state, this optimizer is {self._kind}")
         if sd.get("uncovered") is not None:
             super().load_state_dict(sd["uncovered"])
+        self._load_local_ema(sd)
         for g, saved in zip(self.param_groups, sd["param_groups"]):
             g.update(saved)
         if not self._bucketing.shards:
@@ -185,8 +218,11 @@ class _ShardedStateMixin:
         self._sync_hyper()
 
     def _apply_to_shard(self, rec, sd):
-        for key, t in zip(_STATE_KEYS[self._kind], rec["state"]):
-            per_name = {name: st[key] for name, st in sd["state"].items() if key in st}
+        for key, t in zip(self._state_keys(), rec["state"]):
+            if key == "ema":   # a checkpoint written without an EMA starts it from the loaded master
+                per_name = {name: st["ema"] if "ema" in st else st["master"] for name, st in sd["state"].items() if "ema" in st or "master" in st}
+            else:
+                per_name = {name: st[key] for name, st in sd["state"].items() if key in st}
             t.copy_(shard_of(per_name, rec["layout"], rec["numel"], rec["lo"], rec["hi"], t.numel(), device=t.device))
         for op in rec["step_ops"]:
             op.set_steps(int(sd.get("steps", 0)))
@@ -225,13 +261,19 @@ class _ShardedStateMixin:
 
     def refresh_master_weights(self):
         """Re-read the fp32 master shards from the model weights (call after loading or editing weights without optimizer
-        state: the next bucket kernel writes ``master − lr·update`` over the parameters)."""
+        state: the next bucket kernel writes ``master − lr·update`` over the parameters). With ``ema_decay`` the EMA restarts from the
+        refreshed master: the old average belongs to other weights."""
         if not self._bucketing.shards:
-            return super().refresh_master_weights() if hasattr(super(), "refresh_master_weights") else None
+            out = super().refresh_master_weights() if hasattr(super(), "refresh_master_weights") else None
+            self._restart_local_ema(self._all_params())
+            return out
         for rec in self._bucketing.shards:
             lo, hi = rec["lo"], min(rec["hi"], rec["numel"])
             if hi > lo:
                 rec["state"][0][: hi - lo].copy_(rec["weights"][lo:hi].float())
+            if self._ema:
+                rec["state"][-1].copy_(rec["state"][0])
+        self._restart_local_ema(self._local_ema_params())
 
     def _sync_hyper(self):
         hyper = _HYPER[self._kind]
@@ -259,6 +301,164 @@ class _ShardedStateMixin:
                     torch._foreach_mul_([p.grad for p in left], coef)
                 super().step(only={id(p) for p in left})
             torch._foreach_zero_([p.grad for p in left])
+
+    # ---- exponential moving average of the weights (``ema_decay``) -------------------------------------------------------
+    def _ema_weight(self) -> float:
+        """``w = float(1 − double(ema_decay))``: the host's double difference, rounded once to fp32 by the op."""
+        d = self.ema_decay
+        if d is None or not 0.0 < float(d) < 1.0:
+            raise ValueError(f"ema_decay must be a number in (0, 1), got {d}")
+        return 1.0 - float(d)
+
+    def _ema_source(self, p):
+        """The fp32 weights the EMA of a parameter outside the buckets (or of any parameter on the fallback) follows: its fp32 master,
+        or the parameter itself when it is fp32 (a low-precision one without a master yet: its value, which the master starts from)."""
+        import torch
+
+        m = self.state[p].get("master") if p in self.state else None
+        if m is not None and p.dtype != torch.float32:
+            return m
+        return p.data if p.dtype == torch.float32 else p.data.float()
+
+    def _local_ema_pairs(self, params):
+        """``[(source, ema)]`` of the local EMAs, kept as ``state[p]["ema"]`` in the source's memory layout (the kernel walks raw memory)."""
+        import torch
+
+        pairs = []
+        for p in params:
+            src = self._ema_source(p)
+            if src.stride() != torch.empty_like(src).stride():   # not dense (a view with gaps): the kernel reads a contiguous copy
+                src = src.contiguous()
+            st = self.state[p]
+            e = st.get("ema")
+            if e is None:
+                e = st["ema"] = torch.empty_like(src).copy_(src)
+            elif e.device != src.device or e.dtype != torch.float32 or e.stride() != src.stride():   # e.g. a loaded checkpoint
+                e = st["ema"] = torch.empty_like(src).copy_(e)
+            pairs.append((src, e))
+        return pairs
+
+    def _local_ema_params(self):
+        b = self._bucketing
+        if not b.hyper_ops:
+            return self._all_params()
+        self._uncovered()
+        return b.uncovered
+
+    def _start_local_ema(self):
+        """Before the first update: a local EMA starts from the weights the update begins with, as the bucket shards do."""
+        local = self._local_ema_params()
+        if any("ema" not in self.state[p] for p in local):
+            self._local_ema_pairs(local)
+
+    def _restart_local_ema(self, params):
+        if self._ema:
+            for src, e in self._local_ema_pairs(params or []):
+                e.copy_(src)
+
+    def _run_ema(self, op, stream_device):
+        import torch
+
+        from ...core import native
+
+        op.set_weight(self._ema_weight())
+        native().run_op(op, torch.cuda.current_stream(stream_device).cuda_stream, stream_device.index)
+        self.kernel_launches += 1
+
+    def _local_ema(self, role, params, vote):
+        """One EmaOp launch over the local EMAs of ``params`` (the table is rebuilt only when a pointer changes); on the CPU the same
+        three fp32 roundings in torch."""
+        import torch
+
+        pairs = self._local_ema_pairs(params)
+        if not pairs:
+            return
+        if pairs[0][0].device.type != "cuda":
+            w = torch.tensor(self._ema_weight(), dtype=torch.float32)
+            for src, e in pairs:
+                e.add_(torch.mul(torch.sub(src, e), w))
+            return
+        from ...core import native
+        from ...ops.optim import _cached_plan
+
+        plan = _cached_plan(self._ema_plans, role, [[s for s, _ in pairs], [e for _, e in pairs]])
+        if getattr(plan, "ema_op", None) is None or plan.ema_vote != vote:
+            plan.ema_op, plan.ema_vote = native().EmaOp(*plan.args(), self._ema_weight(), vote), vote
+        self._run_ema(plan.ema_op, pairs[0][0].device)
+
+    def _ema_after_step(self, vote=0):
+        """Every ``ema_every``-th ``step()``: ``e ← e + w·(m − e)`` over every master (one launch for the bucket shards, at most one for
+        the parameters outside the buckets), skipped on the device when the loss-scaled step's vote (``found_inf``) is set."""
+        if not self._ema:
+            return
+        self._ema_calls += 1
+        if self._ema_calls % self.ema_every:
+            return
+        b = self._bucketing
+        if b.hyper_ops:
+            if b.ema is None:
+                raise RuntimeError("the EMA table was not built: not every bucket of the model has been initialised")
+            self._run_ema(b.ema["op"], b.device)
+        self._local_ema("local", self._local_ema_params(), vote)
+
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """Evaluate (or save) the model with its EMA weights: on entry every rank's parameters receive the EMA rounded once to their
+        dtype, on exit the live weights come back bit for bit (the fp32 master is republished, rounded as every update kernel rounds
+        it). A collective: every rank enters and leaves together. ``step()`` inside raises. Buffers (BatchNorm running statistics)
+        are not averaged: they stay the live model's, as with ``AveragedModel(use_buffers=False)``."""
+        import torch
+
+        if not self._ema:
+            raise RuntimeError("this optimizer keeps no EMA; build it with ema_decay=...")
+        if self._ema_swapped:
+            raise RuntimeError("already inside ema_weights()")
+        local = self._local_ema_params()
+        saved = []
+        with torch.no_grad():
+            for p, (_, e) in zip(local, self._local_ema_pairs(local)):   # the local EMAs are swapped in and out with copies
+                saved.append((p, p.data.clone()))
+                p.data.copy_(e)
+            self._ema_publish(0)
+        self._ema_swapped = True
+        try:
+            yield self
+        finally:
+            self._ema_swapped = False
+            with torch.no_grad():
+                self._ema_publish(1)
+                for p, keep in saved:
+                    p.data.copy_(keep)
+
+    def _ema_publish(self, which):
+        """Every bucket's EMA (0) or master (1) shard all-gathered into the weights, one launch per bucket."""
+        import torch
+
+        from ...core import native
+
+        b = self._bucketing
+        if not b.shards:
+            return
+        C, stream, dev = native(), torch.cuda.current_stream(b.device).cuda_stream, b.device.index
+        for rec in b.shards:
+            C.run_op(rec["publish"][which], stream, dev)
+        self.kernel_launches += len(b.shards)
+
+    def ema_state_dict(self):
+        """``{parameter name: full-shape fp32 EMA}`` in the model's parameter order, on the CPU — for saving an averaged model for
+        inference. A collective on the bucket path (an all-gather per bucket), like ``state_dict()``."""
+        if not self._ema:
+            raise RuntimeError("this optimizer keeps no EMA; build it with ema_decay=...")
+        out = {}
+        b = self._bucketing
+        for rec in b.shards:
+            for name, full in consolidate_shards(self._gather(rec["state"][-1], rec["group"]), rec["numel"], rec["layout"]).items():
+                out[name] = full.cpu()
+        local = self._local_ema_params()
+        for i, (p, (_, e)) in enumerate(zip(local, self._local_ema_pairs(local))):
+            out[self._param_names.get(id(p), f"param{i}")] = e.detach().reshape(p.shape).contiguous().cpu().clone()
+        order = {n: i for i, n in enumerate(self._param_names.values())}
+        return dict(sorted(out.items(), key=lambda kv: order.get(kv[0], len(order))))
 
     # ---- global gradient-norm clipping (``max_grad_norm``) ---------------------------------------------------------------
     @property
@@ -355,11 +555,17 @@ class _ShardedStateMixin:
         without a scaler) and votes on overflow: a step whose averaged gradient holds an inf or a NaN changes no weight, no
         optimizer state and not the step count, on any rank (``last_step_skipped``)."""
         b = self._bucketing
+        if self._ema_swapped:
+            raise RuntimeError("step() inside ema_weights(): the parameters hold the EMA, leave the context first")
+        if self._ema:
+            self._start_local_ema()
         if not b.hyper_ops:
             if self.max_grad_norm is not None and not self._norm_pending:
                 self._last_norm = super().clip_grad_norm_(self.max_grad_norm)
             self._norm_pending = False
-            return super().step(closure)
+            out = super().step(closure)
+            self._ema_after_step()
+            return out
         self._sync_hyper()
         coef = found_inf = None
         if b.clip is not None:
@@ -391,6 +597,7 @@ class _ShardedStateMixin:
         self._step_uncovered(coef, found_inf)
         self._grads_zeroed = True
         self.kernel_launches += b.launches
+        self._ema_after_step(found_inf.data_ptr() if found_inf is not None else 0)
         return None
 
     def _register_shard(self, rec):
@@ -416,8 +623,18 @@ def _check_bound(max_grad_norm):
     return None if max_grad_norm is None else float(max_grad_norm)
 
 
+def _set_ema(opt, ema_decay, ema_every):
+    if ema_decay is None:
+        return
+    if not 0.0 < float(ema_decay) < 1.0:
+        raise ValueError(f"ema_decay must be a number in (0, 1) or None, got {ema_decay}")
+    if int(ema_every) != ema_every or int(ema_every) < 1:
+        raise ValueError(f"ema_every must be a positive integer, got {ema_every}")
+    opt._ema, opt.ema_decay, opt.ema_every = True, float(ema_decay), int(ema_every)
+
+
 def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, max_grad_norm=None, loss_scaling=False,
-                           accumulate_grads=False):
+                           accumulate_grads=False, ema_decay=None, ema_every=1):
     """SGD whose update runs *inside* each bucket's NVSwitch kernel (``allreduce_sgd_kernel``): reduce-scatter of the
     gradients → SGD(momentum) on this rank's 1/N shard with fp32 master weights → all-gather of the updated weights, one
     launch per bucket, overlapped with the rest of backward.  Optimizer state is sharded N ways (ZeRO-1-like) and the
@@ -451,6 +668,7 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
     opt = _ShardedFusedSGD(params, lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
                            master_weights=True, zero_grad_in_step=True)
     opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
+    _set_ema(opt, ema_decay, ema_every)
     return opt
 
 
@@ -459,7 +677,7 @@ class ShardedFusedAdam(object):
 
 
 def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False, max_grad_norm=None, loss_scaling=False,
-                            accumulate_grads=False):
+                            accumulate_grads=False, ema_decay=None, ema_every=1):
     """Adam / AdamW counterpart of :func:`make_sharded_fused_sgd`: the update of this rank's 1/N shard (fp32 master weights
     and both moments) runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_adam_kernel``).  With one
     process (or without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedAdam`.  ``max_grad_norm``,
@@ -472,6 +690,7 @@ def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weigh
     opt = _ShardedFusedAdam(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, adamw=adamw, master_weights=True,
                             zero_grad_in_step=True)
     opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
+    _set_ema(opt, ema_decay, ema_every)
     return opt
 
 
@@ -480,7 +699,7 @@ class ShardedFusedLamb(object):
 
 
 def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01, max_grad_norm=None, loss_scaling=False,
-                            accumulate_grads=False):
+                            accumulate_grads=False, ema_decay=None, ema_every=1):
     """LAMB (apex ``FusedLAMB`` semantics, see :class:`bagua_b200.ops.optim.FusedLAMB`) on the in-bucket sharded path: each rank
     keeps fp32 master weights and both moments for its 1/N slice of every bucket.
 
@@ -501,6 +720,7 @@ def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weigh
 
     opt = _ShardedFusedLamb(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, master_weights=True, zero_grad_in_step=True)
     opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
+    _set_ema(opt, ema_decay, ema_every)
     return opt
 
 
@@ -509,7 +729,7 @@ class ShardedFusedLars(object):
 
 
 def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, trust_coefficient=1e-3, max_grad_norm=None, loss_scaling=False,
-                            accumulate_grads=False):
+                            accumulate_grads=False, ema_decay=None, ema_every=1):
     """LARS (see :class:`bagua_b200.ops.optim.FusedLARS`) on the in-bucket sharded path: each rank keeps fp32 master weights and
     the momentum for its 1/N slice of every bucket.
 
@@ -529,6 +749,7 @@ def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, tru
     opt = _ShardedFusedLars(params, lr=lr, momentum=momentum, weight_decay=weight_decay, trust_coefficient=trust_coefficient, master_weights=True,
                             zero_grad_in_step=True)
     opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
+    _set_ema(opt, ema_decay, ema_every)
     return opt
 
 
@@ -553,6 +774,8 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
             if sharded and opt._bucketing.hyper_ops:
                 opt._sync_hyper()
 
+        if sharded and opt._ema:   # the names ema_state_dict() gives the local EMAs
+            opt._param_names = {id(p): name for name, p in bagua_ddp.module.named_parameters()}
         # _reset_buckets builds this hook after the last init_operations: every new shard has consumed the carried-over state
         # (checkpoint loaded before with_bagua, or the snapshot taken in tensors_to_buckets) — it must not be applied again
         opt._pending_state = None
@@ -694,6 +917,12 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         rec = {"bucket": bucket.name, "group": self.process_group, "numel": flat.numel(), "lo": lo, "hi": hi, "layout": layout,
                "state": (master, momentum, second) if is_adam or is_lamb else (master, momentum), "weights": wflat,
                "param_ids": [id(t) for t in bucket.tensors], "shard": None}
+        if opt._ema:
+            # the EMA shard starts equal to the master (a carried-over or loaded state overwrites both); publishing it, or the master
+            # back, is one launch per bucket on entry to and exit from ema_weights()
+            ema = master.clone()
+            rec["state"] += (ema,)
+            rec["publish"] = tuple(C.ShardPublishOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, src.data_ptr(), use_mc, cfg) for src in (ema, master))
         bk.device = flat.device
         if two_phase:
             # phase A in the bucket program: reduce-scatter into the fp32 shard (added to it when accumulating) + per-CTA Σx² into
@@ -743,6 +972,13 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         bk.launches += len(rec["step_ops"])
         opt._register_shard(rec)
         opt._sync_hyper()
+        if opt._ema and len(bk.shards) == len(bagua_ddp.bagua_buckets):
+            # one launch per step over every bucket's [master, EMA] pair; with loss scaling it obeys the vote on the device
+            from ...ops.optim import multi_tensor_plan
+
+            plan = multi_tensor_plan([[r["state"][0] for r in bk.shards], [r["state"][-1] for r in bk.shards]])
+            vote = bk.clip["out"][2:].data_ptr() if scaled else 0
+            bk.ema = {"plan": plan, "op": C.EmaOp(*plan.args(), opt._ema_weight(), vote)}
 
     def _per_param_state(self, eng, bagua_ddp, bucket, device):
         """State of the per-parameter exchange of LAMB and LARS (LambRatioOp), shared by all buckets: a global index of the bucketed
@@ -777,7 +1013,7 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         C = native()
         lam = bk.lamb
         master, shard, lo, hi, dev = rec["state"][0], rec["shard"], rec["lo"], rec["hi"], bk.device
-        lists = (master, shard) if lars else (master, shard) + tuple(rec["state"][1:])
+        lists = (master, shard) if lars else (master, shard) + tuple(rec["state"][1:3])
         Stage1 = C.LarsNormsOp if lars else C.LambMomentsOp
         segs, views = [], [[] for _ in lists]
         for name, off, n, _, _ in rec["layout"]:

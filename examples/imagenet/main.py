@@ -72,6 +72,9 @@ def parse():
     p.add_argument("--optimizer", default="sgd", choices=["sgd", "lars"], help="momentum SGD, or LARS for large global batches (BatchNorm "
                    "and bias parameters get no weight decay and no layer adaptation)")
     p.add_argument("--trust-coefficient", type=float, default=1e-3, help="LARS trust coefficient (eta)")
+    p.add_argument("--ema-decay", type=float, default=None, help="with --fused-shard: keep a sharded fp32 EMA of the weights with this decay; "
+                   "validation then also reports the EMA weights' accuracy, and checkpoints carry the EMA in the optimizer state")
+    p.add_argument("--ema-every", type=int, default=1, help="update the EMA on every N-th optimizer step")
     p.add_argument("--fuse-optimizer", action="store_true", help="generic fused optimizer (bagua.contrib.fuse_optimizer)")
     p.add_argument("--synthetic", action="store_true")
     p.add_argument("--steps-per-epoch", type=int, default=100, help="synthetic data only")
@@ -80,6 +83,8 @@ def parse():
     p.add_argument("--cpu", action="store_true")
     args = p.parse_args()
     args.data = args.data or args.data_pos
+    if args.ema_decay is not None and not args.fused_shard:
+        p.error("--ema-decay needs --fused-shard")
     args.milestone_list = sorted(int(m) for m in args.milestones.split(",") if m.strip())
     return args
 
@@ -167,12 +172,14 @@ def make_optimizer(args, model, lr, cuda, world):
         groups = [{"params": [p for p in model.parameters() if p.dim() > 1], "weight_decay": args.weight_decay},
                   {"params": [p for p in model.parameters() if p.dim() <= 1], "weight_decay": 0.0}]
         kw = dict(lr=lr, momentum=args.momentum, trust_coefficient=args.trust_coefficient)
-        if args.fused_shard and cuda:
-            opt = make_sharded_fused_lars(groups, **kw)
+        if args.fused_shard and (cuda or args.ema_decay is not None):
+            opt = make_sharded_fused_lars(groups, ema_decay=args.ema_decay, ema_every=args.ema_every, **kw)
             return opt, FusedGradientAllReduceAlgorithm(opt)
         return bagua.ops.FusedLARS(groups, **kw), Algorithm.init(args.algorithm)
-    if args.fused_shard and cuda and args.algorithm == "gradient_allreduce":
-        opt = make_sharded_fused_sgd(model.parameters(), lr=lr, momentum=args.momentum, weight_decay=args.weight_decay)
+    # with --ema-decay also on the CPU: the sharded optimizer's fallback keeps the EMA there
+    if args.fused_shard and (cuda or args.ema_decay is not None) and args.algorithm == "gradient_allreduce":
+        opt = make_sharded_fused_sgd(model.parameters(), lr=lr, momentum=args.momentum, weight_decay=args.weight_decay, ema_decay=args.ema_decay,
+                                     ema_every=args.ema_every)
         return opt, FusedGradientAllReduceAlgorithm(opt)
     if cuda and not args.fuse_optimizer:
         opt = bagua.ops.FusedSGD(model.parameters(), lr=lr, momentum=args.momentum, weight_decay=args.weight_decay)   # one multi-tensor kernel per step
@@ -248,8 +255,16 @@ def main():
     def nvtx(name):
         return torch.cuda.nvtx.range(name) if (cuda and args.prof >= 0) else contextlib.nullcontext()
 
-    @torch.no_grad()
     def validate(epoch):
+        """Acc@1 of the live weights and, with --ema-decay, of the EMA weights (BatchNorm statistics stay the live model's)."""
+        acc1 = score(epoch, "")
+        if args.ema_decay is not None:
+            with optimizer.ema_weights():   # collective: every rank validates its shard of the set
+                score(epoch, "EMA ")
+        return acc1
+
+    @torch.no_grad()
+    def score(epoch, label):
         model.eval()
         tot = torch.zeros(4, device=dev)   # top-1 hits, top-5 hits, samples, summed loss
         t0 = time.time()
@@ -262,7 +277,7 @@ def main():
                 logging.info("Test: [%d/%d]\tTime %.3f", i, len(val_loader), time.time() - t0)
         bagua.allreduce_inplace(tot, op=bagua.ReduceOp.SUM)   # every rank scored its own shard of the validation set
         acc1, acc5 = (100.0 * tot[0] / tot[2]).item(), (100.0 * tot[1] / tot[2]).item()
-        logging.info(" * Epoch %d Acc@1 %.3f Acc@5 %.3f Loss %.4f", epoch, acc1, acc5, (tot[3] / tot[2]).item())
+        logging.info(" * Epoch %d %sAcc@1 %.3f %sAcc@5 %.3f Loss %.4f", epoch, label, acc1, label, acc5, (tot[3] / tot[2]).item())
         return acc1
 
     def train(epoch):

@@ -145,7 +145,15 @@ for acc, nb in ((False, 6), (True, 10)):
     sg = C.ShardGradOp(comm, a.buf, 0, NB, code, shard.data_ptr(), gpart.data_ptr(), 1.0, True, False, w.cfg(64), acc)
     run(sg)   # an accumulating op overwrites on its first run
     timed(f"shard_grad_kernel<bf16,P=1,peer,ACCUM={str(acc).lower()}> 64MiB bucket", lambda sg=sg: run(sg), n * nb)
-del shard, lpart, npart, gpart
+# weight EMA of the same shard: the local update (reads master and EMA 8B, writes the EMA 4B per element), and the EMA published as the
+# bucket's weights (reads the shard 4B, writes the weights 2B per element)
+eshard = master.clone()
+eplan = multi_tensor_plan([[master], [eshard]])
+ema_op = C.EmaOp(*eplan.args(), 1e-4, 0)
+timed("multi_tensor_ema_kernel 32M-element shard", lambda: run(ema_op), n * 12)
+pub = C.ShardPublishOp(comm, b.buf, 0, NB, code, eshard.data_ptr(), False, w.cfg(64))
+timed("shard_publish_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(pub), n * 6)
+del shard, lpart, npart, gpart, eshard
 
 # single-GPU kernels ------------------------------------------------------------------------------------------------------
 P = 138 * 1000 * 1000 // 8 * 8   # VGG16-sized arena
