@@ -20,7 +20,7 @@ def _live(optimizer) -> bool:
 
 
 class ShardedGradScaler(GradScaler):
-    """``torch.amp.GradScaler`` (device ``"cuda"``) that can drive ``make_sharded_fused_{sgd,adam,lamb,lars}(loss_scaling=True)``::
+    """``torch.amp.GradScaler`` (device ``"cuda"``) that can drive ``make_sharded_fused_{sgd,adam,lamb,lars,lion}(loss_scaling=True)``::
 
         scaler.scale(loss).backward()
         scaler.step(opt)        # no host synchronisation while the bucket kernels are live
@@ -61,7 +61,7 @@ class ShardedGradScaler(GradScaler):
             return super().step(optimizer, *args, **kwargs)
         if not optimizer.loss_scaling:
             raise RuntimeError("this in-bucket optimizer applied the update during backward, with the still-scaled gradients: a step that "
-                               "overflowed can no longer be skipped. Build it with loss_scaling=True (make_sharded_fused_sgd / _adam / _lamb / _lars)")
+                               "overflowed can no longer be skipped. Build it with loss_scaling=True (make_sharded_fused_sgd / _adam / _lamb / _lars / _lion)")
         if "closure" in kwargs or args:
             raise RuntimeError("Closure use is not currently supported if GradScaler is enabled.")
         self._check_scale_growth_tracker("step")

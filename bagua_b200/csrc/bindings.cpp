@@ -304,6 +304,16 @@ PYBIND11_MODULE(_C, m) {
                  py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
                  py::arg("master_ptr"), py::arg("momentum_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("sums_ptr"), py::arg("use_multimem"),
                  py::arg("cfg")));
+    def_stepped<AllReduceLionOp, double, double, double, double>(
+        py::class_<AllReduceLionOp, CommOp, std::shared_ptr<AllReduceLionOp>>(m, "AllReduceLionOp")
+            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, SymmBuf, size_t, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool, LaunchCfg>(),
+                 py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"),
+                 py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg")));
+    def_stepped<ShardLionOp, double, double, double, double>(
+        py::class_<ShardLionOp, CommOp, std::shared_ptr<ShardLionOp>>(m, "ShardLionOp")
+            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(),
+                 py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
+                 py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("use_multimem"), py::arg("cfg")));
     py::class_<EmaOp, CommOp, std::shared_ptr<EmaOp>>(m, "EmaOp")
         .def(py::init<uint64_t, uint64_t, uint64_t, uint64_t, int, int, int, float, uint64_t>(), py::arg("ptrs"), py::arg("sizes"), py::arg("b2t"),
              py::arg("b2c"), py::arg("n_tensors"), py::arg("n_blocks"), py::arg("chunk"), py::arg("weight"), py::arg("vote_ptr"))
@@ -425,6 +435,13 @@ PYBIND11_MODULE(_C, m) {
                                reinterpret_cast<const int32_t*>(b2t), reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk};
               launch_multi_tensor_lars_stage2(d, dtype, mixed, LarsParams{lr, momentum, wd, trust_coefficient}, reinterpret_cast<const float*>(coef),
                                               reinterpret_cast<const double*>(sums), zero_grad, S(stream));
+          });
+    m.def("multi_tensor_lion",
+          [](uint64_t ptrs, uint64_t sizes, uint64_t b2t, uint64_t b2c, int n_tensors, int n_blocks, int chunk, int dtype, bool mixed, double lr,
+             double beta1, double beta2, double wd, bool zero_grad, uint64_t stream) {
+              TensorListDesc d{reinterpret_cast<const uint64_t*>(ptrs), reinterpret_cast<const int64_t*>(sizes),
+                               reinterpret_cast<const int32_t*>(b2t), reinterpret_cast<const int32_t*>(b2c), n_tensors, n_blocks, chunk};
+              launch_multi_tensor_lion(d, dtype, mixed, lion_params(lr, beta1, beta2, wd), zero_grad, S(stream));
           });
     m.def("qadam_momentum", [](uint64_t m1, uint64_t grad, int gdt, size_t n, float beta1, uint64_t stream) {
         launch_qadam_momentum(reinterpret_cast<float*>(m1), reinterpret_cast<const void*>(grad), gdt, n, beta1, S(stream));

@@ -55,6 +55,22 @@ struct LarsParams {
     float trust_coefficient;
 };
 
+// Lion (Chen et al. 2023, Algorithm 2) as fp32 constants, each worked out in double from the group's hyper-parameters and rounded
+// once (lion_params): b1 = β1, c1 = 1 − β1, b2 = β2, c2 = 1 − β2, d = 1 − lr·wd (see lion.cuh). No step-dependent field.
+struct LionParams {
+    float lr;
+    float b1;
+    float c1;
+    float b2;
+    float c2;
+    float d;
+};
+
+inline LionParams lion_params(double lr, double beta1, double beta2, double weight_decay) {
+    return LionParams{static_cast<float>(lr), static_cast<float>(beta1), static_cast<float>(1.0 - beta1), static_cast<float>(beta2),
+                      static_cast<float>(1.0 - beta2), static_cast<float>(1.0 - lr * weight_decay)};
+}
+
 // 1 - beta^step of the in-bucket Adam and LAMB ops and of FusedLAMB: in double, rounded once. Also callable from device code: the
 // kernels that take the step count from device memory (loss scaling) build their bias corrections with it.
 #ifdef __CUDACC__
@@ -135,6 +151,15 @@ void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off,
 void launch_shard_lars(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
                        float* master, float* momentum, const int32_t* segs, int nsegs, const double* sums, const LarsParams& hp, bool use_multimem,
                        int nblocks, int nthreads, cudaStream_t stream, bool vote = false);
+// In-bucket Lion (lion.cuh). allreduce_lion: the walk of launch_allreduce_adam with g = fl(red·scale), the fp32 master and exp_avg
+// of the owned shard. shard_lion: phase B over the fp32 gradient shard with g = fl(shard·*coef); with `vote` coef addresses
+// {coef, found_inf} and a found_inf step touches no state and only takes the closing barrier.
+void launch_allreduce_lion(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
+                           float* master, float* exp_avg, const LionParams& hp, float scale, bool zero_grads, bool use_multimem, int nblocks, int nthreads,
+                           cudaStream_t stream);
+void launch_shard_lion(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                       float* master, float* exp_avg, const LionParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream,
+                       bool vote = false);
 // Weight EMA of the in-bucket optimizers: publishes the fp32 shard `src` (the owned slice, shard-local like the master) rounded with
 // Vec16<T>::pack into every rank's copy of the weights, between an opening and a closing barrier. preload_shard_publish loads the
 // instantiation for one dtype / world / flavour.
@@ -281,6 +306,9 @@ void launch_multi_tensor_lamb_stage2(const TensorListDesc& d, int dtype, bool mi
 void launch_multi_tensor_lars_stage1(const TensorListDesc& d, int dtype, bool mixed, const float* coef, double* sums, cudaStream_t stream, bool vote = false);
 void launch_multi_tensor_lars_stage2(const TensorListDesc& d, int dtype, bool mixed, const LarsParams& hp, const float* coef, const double* sums, bool zero_grad,
                                      cudaStream_t stream);
+// Lion in one launch, lists [param(T), grad(T), (master(f32) when mixed,) exp_avg(f32)]: lion.cuh's update with g = grad; mixed writes
+// the fp32 master and the parameter rounded once; the gradient is cleared in the same pass when zero_grad.
+void launch_multi_tensor_lion(const TensorListDesc& d, int dtype, bool mixed, const LionParams& hp, bool zero_grad, cudaStream_t stream);
 // Exponential moving average of fp32 weights, lists [source(f32), ema(f32)]: e ← fl(e + fl(w·fl(m − e))), three separately rounded
 // operations. `vote` (nullable): with *vote != 0 (an overflowed loss-scaled step) nothing is written.
 void launch_multi_tensor_ema(const TensorListDesc& d, float weight, const float* vote, cudaStream_t stream);

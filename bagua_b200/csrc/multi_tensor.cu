@@ -13,6 +13,7 @@
 #include "kernels.h"
 #include "lamb.cuh"
 #include "lars.cuh"
+#include "lion.cuh"
 #include "quant.cuh"
 
 namespace bagua {
@@ -569,6 +570,39 @@ void launch_multi_tensor_lars_stage2(const TensorListDesc& d, int dtype, bool mi
         });
     });
     check_launch("multi_tensor_lars_stage2");
+}
+
+// ---- Lion: one pass, the gradient cleared on the way ---------------------------------------------------------------------
+// lists = [param(T), grad(T), (master(f32) when MIXED,) exp_avg(f32)]; the update is lion.cuh's, with coef 1.
+template <typename T, bool MIXED>
+__global__ void __launch_bounds__(kThreads) multi_tensor_lion_kernel(TensorListDesc d, LionParams hp, int zero_grad) {
+    const int t = d.block_to_tensor[blockIdx.x];
+    const size_t off = static_cast<size_t>(d.block_to_chunk[blockIdx.x]) * d.chunk;
+    const size_t n = static_cast<size_t>(d.sizes[t]);
+    const size_t len = (n - off) < static_cast<size_t>(d.chunk) ? (n - off) : static_cast<size_t>(d.chunk);
+    T* p = reinterpret_cast<T*>(d.ptrs[t]) + off;
+    T* g = reinterpret_cast<T*>(d.ptrs[d.n_tensors + t]) + off;
+    float* mw = MIXED ? reinterpret_cast<float*>(d.ptrs[2 * d.n_tensors + t]) + off : nullptr;
+    float* ea = reinterpret_cast<float*>(d.ptrs[(MIXED ? 3 : 2) * d.n_tensors + t]) + off;
+    for (size_t i = threadIdx.x; i < len; i += blockDim.x) {
+        float w = MIXED ? mw[i] : to_f32<T>(p[i]), m = ea[i];
+        lion_apply(w, m, lion_grad(to_f32<T>(g[i]), 1.f), hp);
+        ea[i] = m;
+        if (MIXED) mw[i] = w;
+        p[i] = from_f32<T>(w);
+        if (zero_grad) g[i] = from_f32<T>(0.f);
+    }
+}
+
+void launch_multi_tensor_lion(const TensorListDesc& d, int dtype, bool mixed, const LionParams& hp, bool zero_grad, cudaStream_t stream) {
+    if (d.n_blocks <= 0) return;
+    dispatch_float(dtype, "optimizer kernels", [&](auto tag) {
+        using T = decltype(tag);
+        dispatch_flag(mixed, [&](auto mx) {
+            multi_tensor_lion_kernel<T, decltype(mx)::value><<<d.n_blocks, kThreads, 0, stream>>>(d, hp, zero_grad ? 1 : 0);
+        });
+    });
+    check_launch("multi_tensor_lion");
 }
 
 // ---- exponential moving average of fp32 weights ---------------------------------------------------------------------

@@ -229,6 +229,22 @@ void ShardLarsOp::run(Bucket&, StreamHandle stream, int) {
     steps_++;
 }
 
+void AllReduceLionOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("allreduce_lion");
+    if (vote()) throw std::runtime_error("bagua: allreduce_lion updates during backward and cannot obey a device-side vote");
+    launch_allreduce_lion(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_),
+                          reinterpret_cast<float*>(exp_avg_), params(), scale_, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
+    steps_++;
+}
+
+void ShardLionOp::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal("shard_lion");
+    launch_shard_lion(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), coef_or_vote(coef_),
+                      reinterpret_cast<float*>(master_), reinterpret_cast<float*>(exp_avg_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream),
+                      vote() != nullptr);
+    steps_++;
+}
+
 void EmaOp::run(Bucket&, StreamHandle stream, int) { launch_multi_tensor_ema(desc_, weight(), reinterpret_cast<const float*>(vote_), S(stream)); }
 
 ShardPublishOp::ShardPublishOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t src, bool use_multimem,

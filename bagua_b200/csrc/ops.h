@@ -130,6 +130,10 @@ struct LambHyper {
 struct LarsHyper {
     float lr = 1e-3f, momentum = 0.9f, weight_decay = 0.f, trust_coefficient = 1e-3f;
 };
+// in double: the kernel's constants are worked out from these and rounded once (lion_params)
+struct LionHyper {
+    double lr = 1e-4, beta1 = 0.9, beta2 = 0.99, weight_decay = 0.0;
+};
 
 // What a rule's kernel receives at the launch that follows `steps` earlier ones.
 inline SgdParams device_params(const SgdHyper& h, uint64_t steps) {
@@ -140,6 +144,7 @@ inline AdamParams device_params(const AdamHyper& h, uint64_t steps) {
 }
 inline LambParams device_params(const LambHyper& h, uint64_t steps) { return lamb_params(h.lr, h.beta1, h.beta2, h.eps, h.weight_decay, steps + 1); }
 inline LarsParams device_params(const LarsHyper& h, uint64_t) { return LarsParams{h.lr, h.momentum, h.weight_decay, h.trust_coefficient}; }
+inline LionParams device_params(const LionHyper& h, uint64_t) { return lion_params(h.lr, h.beta1, h.beta2, h.weight_decay); }
 
 // An optimizer op: hyper-parameters published from Python (the forward pre-hook may do so while the comm worker runs the op, hence
 // the lock) and the count of launches so far, which checkpoints save and restore. With loss scaling a launch may be a skipped step,
@@ -474,6 +479,48 @@ private:
     uint64_t shard_, coef_, master_, momentum_, segs_;
     int nsegs_;
     uint64_t sums_;
+    bool use_mc_;
+    LaunchCfg cfg_;
+};
+
+// In-bucket Lion. AllReduceLionOp is the Lion flavour of the fused bucket op (update during backward); ShardLionOp is phase B of the
+// two-phase program (after ShardGradOp), the gradient shard·*coef. Lion's kernel arguments hold only the hyper-parameters, which do
+// not depend on the step, so both ops are step-invariant; they count their launches for checkpoints like every optimizer op.
+class AllReduceLionOp final : public SteppedOp<LionHyper> {
+public:
+    AllReduceLionOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, SymmBuf weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
+                    uint64_t master, uint64_t exp_avg, float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), grads_(grads), weights_(weights), g_off_(g_off), w_off_(w_off), bytes_(bytes), dtype_(dtype),
+          master_(master), exp_avg_(exp_avg), scale_(scale), zero_grads_(zero_grads), use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return "allreduce_lion"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf grads_, weights_;
+    size_t g_off_, w_off_, bytes_;
+    int dtype_;
+    uint64_t master_, exp_avg_;
+    const float scale_;
+    bool zero_grads_, use_mc_;
+    LaunchCfg cfg_;
+};
+
+class ShardLionOp final : public SteppedOp<LionHyper> {
+public:
+    ShardLionOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
+                uint64_t exp_avg, bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), master_(master),
+          exp_avg_(exp_avg), use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return "shard_lion"; }
+    void run(Bucket&, StreamHandle stream, int device) override;
+
+private:
+    std::shared_ptr<PeerComm> comm_;
+    SymmBuf weights_;
+    size_t w_off_, bytes_;
+    int dtype_;
+    uint64_t shard_, coef_, master_, exp_avg_;
     bool use_mc_;
     LaunchCfg cfg_;
 };

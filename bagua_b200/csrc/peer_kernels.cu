@@ -8,6 +8,7 @@
 #include "kernels.h"
 #include "lamb.cuh"
 #include "lars.cuh"
+#include "lion.cuh"
 #include "peer.cuh"
 
 namespace bagua {
@@ -359,6 +360,53 @@ __global__ void __launch_bounds__(512)
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// Lion on one 16-byte vector of the owned shard (lion.cuh): x[k]·coef is the gradient, the fp32 master and exp_avg are updated in
+// place and w receives the new weights, which the caller publishes.
+// ---------------------------------------------------------------------------------------------------------
+template <int N>
+__device__ __forceinline__ void lion_update(float* master, float* exp_avg, size_t j, const float* x, float coef, const LionParams& hp, float* w) {
+    float4* wp = reinterpret_cast<float4*>(master + j * N);
+    float4* mp = reinterpret_cast<float4*>(exp_avg + j * N);
+#pragma unroll
+    for (int q = 0; q < N / 4; ++q) {
+        const float4 ww = wp[q], mm = mp[q];
+        float wv[4] = {ww.x, ww.y, ww.z, ww.w}, mv[4] = {mm.x, mm.y, mm.z, mm.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            lion_apply(wv[k], mv[k], lion_grad(x[4 * q + k], coef), hp);
+            w[4 * q + k] = wv[k];
+        }
+        wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
+        mp[q] = make_float4(mv[0], mv[1], mv[2], mv[3]);
+    }
+}
+
+// The reduce-scatter → optimizer → all-gather kernel of allreduce_adam_kernel with Lion on the owned shard (fp32 master weights and
+// exp_avg sharded P ways): one moment instead of two, so 16 bytes of state per owned element instead of 24.
+template <typename T, int P, bool USE_MC>
+__global__ void __launch_bounds__(512)
+    allreduce_lion_kernel(PeerCtx ctx, PeerBuf grads, PeerBuf weights, size_t g_off, size_t w_off, size_t total_vecs, float* master, float* exp_avg,
+                          LionParams hp, float scale, int zero_grads) {
+    const uint32_t e0 = load_epoch(ctx);
+    bool ok = peer_barrier(ctx, e0 + 1);
+    constexpr int N = Vec16<T>::N;
+    const Slicing sl(total_vecs, P);
+    if (ok) {
+        reduce_owned_slice<T, P, USE_MC, kOptimizerUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t v, size_t j, float* g) {
+            float w[N];
+            lion_update<N>(master, exp_avg, j, g, scale, hp, w);
+            publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
+        });
+        ok = peer_barrier(ctx, e0 + 2);
+    }
+    if (ok && zero_grads) {
+        char* mine = grads.ptr[ctx.rank] + g_off;
+        for_each_striped<P>(sl, [&](size_t v) { st_stream16(mine + v * 16, make_uint4(0, 0, 0, 0)); });
+    }
+    store_epoch(ctx, e0 + 2);
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // Global-norm gradient clipping for the in-bucket optimizers. No shard may be updated before the norm over every bucket of every
 // rank is known, so the single in-bucket kernel above becomes two phases around a norm exchange:
 //   A  shard_grad_kernel, per bucket, inside backward on the comm stream: the owned-slice reduction (same order and the same
@@ -616,6 +664,23 @@ __global__ void __launch_bounds__(512) shard_adam_kernel(PeerCtx ctx, PeerBuf we
             adam_update<Vec16<T>::N>(master, exp_avg, exp_avg_sq, j, g, c, hp, inv_bc1, inv_sqrt_bc2, w);
         });
     }
+    peer_barrier(ctx, e0 + 1);
+    store_epoch(ctx, e0 + 1);
+}
+
+// Phase B of the in-bucket Lion: the update of the owned shard from the gradient shard·*coef. Lion has no step-dependent parameter,
+// so loss scaling needs only the vote: with VOTE coef addresses {coef, found_inf} and a skipped step touches no state, publishes
+// nothing and only takes the closing barrier.
+template <typename T, int P, bool USE_MC, bool VOTE>
+__global__ void __launch_bounds__(512) shard_lion_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
+                                                         const float* coef, float* master, float* exp_avg, LionParams hp) {
+    const uint32_t e0 = load_epoch(ctx);
+    const float c = *coef;
+    bool skip = false;
+    if constexpr (VOTE) skip = coef[1] != 0.f;
+    if (!skip)
+        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard,
+                                         [&](size_t j, const float* g, float* w) { lion_update<Vec16<T>::N>(master, exp_avg, j, g, c, hp, w); });
     peer_barrier(ctx, e0 + 1);
     store_epoch(ctx, e0 + 1);
 }
@@ -1078,6 +1143,40 @@ void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerB
         });
     });
     check_launch("allreduce_adam");
+}
+
+void launch_allreduce_lion(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
+                           float* master, float* exp_avg, const LionParams& hp, float scale, bool zero_grads, bool use_multimem, int nblocks, int nthreads,
+                           cudaStream_t stream) {
+    const size_t vecs = peer_vecs("allreduce_lion", bytes, g_off, w_off, nblocks);
+    if (vecs == 0) return;
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(ctx.world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                allreduce_lion_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
+                    ctx, grads, weights, g_off, w_off, vecs, master, exp_avg, hp, scale, zero_grads ? 1 : 0);
+            });
+        });
+    });
+    check_launch("allreduce_lion");
+}
+
+void launch_shard_lion(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                       float* master, float* exp_avg, const LionParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream, bool vote) {
+    const size_t vecs = peer_vecs("shard_lion", bytes, w_off, 0, nblocks);
+    if (coef == nullptr) throw std::runtime_error("bagua: shard_lion needs a gradient coefficient ({coef, found_inf} with a vote)");
+    if (vecs == 0) return;
+    dispatch_float(dtype, kFamily, [&](auto tag) {
+        dispatch_world(ctx.world, [&](auto pw) {
+            dispatch_mc(use_multimem, [&](auto mc) {
+                dispatch_flag(vote, [&](auto vt) {
+                    shard_lion_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(vt)::value><<<nblocks, nthreads, 0, stream>>>(
+                        ctx, weights, w_off, vecs, shard, coef, master, exp_avg, hp);
+                });
+            });
+        });
+    });
+    check_launch("shard_lion");
 }
 
 void launch_shard_grad(const PeerCtx& ctx, const PeerBuf& grads, size_t g_off, size_t bytes, int dtype, float* shard, double* partials, float scale,

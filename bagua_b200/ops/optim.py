@@ -16,7 +16,7 @@ import torch
 from ..core import dtype_code, native
 from ..tensor import dense_strides
 
-__all__ = ["FusedSGD", "FusedAdam", "FusedLAMB", "FusedLARS", "flat_sgd_", "flat_adam_", "multi_tensor_plan"]
+__all__ = ["FusedSGD", "FusedAdam", "FusedLAMB", "FusedLARS", "FusedLion", "flat_sgd_", "flat_adam_", "multi_tensor_plan"]
 
 
 def _stream() -> int:
@@ -705,3 +705,107 @@ class FusedLARS(_FusedBase):
             v = st["momentum_buffer"]
             v.mul_(mom).add_(g + wd * w, alpha=lt)
             p.data.copy_(w - v)
+
+
+def _lion_constants(lr, betas, weight_decay):
+    """Lion's fp32 constants ``(lr, b1, c1, b2, c2, d)`` as the kernels receive them: each worked out in double, rounded once."""
+    b1, b2 = float(betas[0]), float(betas[1])
+    vals = (float(lr), b1, 1.0 - b1, b2, 1.0 - b2, 1.0 - float(lr) * float(weight_decay))
+    return tuple(torch.tensor(v, dtype=torch.float32) for v in vals)
+
+
+def _lion_sign(u: torch.Tensor) -> torch.Tensor:
+    """+1 / −1, +0 for ±0 and NaN for NaN (``torch.sign`` maps NaN to 0, which would make a NaN gradient a silent no-op)."""
+    return torch.where(torch.isnan(u), u, torch.sign(u))
+
+
+def lion_reference_step_(w: torch.Tensor, m: torch.Tensor, x: torch.Tensor, lr, betas, weight_decay, coef=None):
+    """One Lion step in torch fp32, in place on ``w`` and ``m`` (fp32 tensors), ``x`` the gradient and ``coef`` (optional fp32 0-d
+    tensor) its coefficient. Every product and sum is a separate fp32 op, so it reproduces the kernels bit for bit (see lion.cuh)."""
+    lr32, b1, c1, b2, c2, d = (t.to(w.device) for t in _lion_constants(lr, betas, weight_decay))
+    g = x.float() if coef is None else torch.mul(x.float(), coef.to(w.device, torch.float32))
+    u = torch.add(torch.mul(b1, m), torch.mul(c1, g))
+    w.copy_(torch.sub(torch.mul(w, d), torch.mul(lr32, _lion_sign(u))))
+    m.copy_(torch.add(torch.mul(b2, m), torch.mul(c2, g)))
+
+
+class FusedLion(_FusedBase):
+    """Lion (Chen et al., 2023, "Symbolic Discovery of Optimization Algorithms", Algorithm 2), one multi-tensor kernel per dtype
+    group and step, the gradient cleared in the same pass.
+
+    ``u = β1·m + (1−β1)·g``, ``w ← w·(1 − lr·wd) − lr·sign(u)``, ``m ← β2·m + (1−β2)·g``: every element moves by exactly ±lr (0 where
+    ``u`` is 0, NaN where it is NaN), after the decoupled weight decay. One fp32 moment per element (``exp_avg``), half of Adam's
+    state. The constants are worked out in double and rounded to fp32 once, and every product and sum is rounded separately, so
+    the CPU implementation (``_torch_step``, used for CPU tensors) gives the same bits as the kernel. ``master_weights=True`` keeps
+    fp32 master weights for bf16/fp16 parameters and writes the parameter rounded once. Lion wants a smaller ``lr`` and a larger
+    ``weight_decay`` than AdamW (the paper suggests 3–10× and 3–10×)."""
+
+    def __init__(self, params, lr=1e-4, betas=(0.9, 0.99), weight_decay=0.0, master_weights=True, zero_grad_in_step=True):
+        if not 0.0 <= lr:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if not 0.0 <= weight_decay:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        for i, b in enumerate(betas):
+            if not 0.0 <= b < 1.0:
+                raise ValueError(f"Invalid beta parameter at index {i}: {b}")
+        defaults = dict(lr=lr, betas=betas, weight_decay=weight_decay)
+        super().__init__(params, defaults, master_weights, zero_grad_in_step)
+
+    @torch.no_grad()
+    def step(self, closure=None, only: Optional[set] = None):
+        """``only``: see :meth:`FusedSGD.step`."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        C = native()
+        for gi, group in enumerate(self.param_groups):
+            lr, (b1, b2), wd = group["lr"], group["betas"], group["weight_decay"]
+            params = [p for p in group["params"] if p.grad is not None and (only is None or id(p) in only)]
+            if not params:
+                continue
+            if not _kernels_apply(params):
+                self._torch_step(params, group)
+                continue
+            for p in params:
+                st = self.state[p]
+                m = st.get("exp_avg")
+                if m is None:   # fp32 moment in the parameter's memory order (the kernel walks raw memory)
+                    st["exp_avg"] = torch.zeros_like(p.data, dtype=torch.float32)
+                elif m.dtype != torch.float32 or m.stride() != p.stride():   # e.g. a checkpoint written with another layout
+                    st["exp_avg"] = torch.empty_like(p.data, dtype=torch.float32).copy_(m)
+                if self.master_weights and p.dtype in (torch.float16, torch.bfloat16) and "master" not in st:
+                    st["master"] = torch.empty_like(p.data, dtype=torch.float32).copy_(p.data)
+            for (dt, k), ps in _launch_groups(params, lambda p: 0):
+                mixed = self.master_weights and dt in (torch.float16, torch.bfloat16)
+                grads = [_grad_in_layout(p, dt) for p in ps]
+                lists = [[p.data for p in ps], grads]
+                if mixed:
+                    lists.append([self.state[p]["master"] for p in ps])
+                lists.append([self.state[p]["exp_avg"] for p in ps])
+                plan = _cached_plan(self._multi, (gi, dt, k), lists)
+                C.multi_tensor_lion(*plan.args(), dtype_code(dt), mixed, float(lr), float(b1), float(b2), float(wd), bool(self.zero_grad_in_step),
+                                    _stream())
+                self.kernel_launches += 1
+                if self.zero_grad_in_step:
+                    for p, g in zip(ps, grads):
+                        if g is not p.grad:   # the kernel cleared a converted copy
+                            p.grad.zero_()
+        if only is None:
+            self._grads_zeroed = self.zero_grad_in_step
+        return loss
+
+    def _torch_step(self, params, group):
+        """The same rule in torch fp32 (CPU tensors), bit for bit."""
+        for p in params:
+            st = self.state[p]
+            if "exp_avg" not in st:
+                st["exp_avg"] = torch.zeros_like(p.data, dtype=torch.float32)
+            lowp = p.dtype != torch.float32
+            if lowp and self.master_weights and "master" not in st:
+                st["master"] = p.data.float()
+            w = st["master"] if lowp and self.master_weights else p.data.float()
+            lion_reference_step_(w, st["exp_avg"], p.grad, group["lr"], group["betas"], group["weight_decay"])
+            p.data.copy_(w)
+            if self.zero_grad_in_step:
+                p.grad.zero_()

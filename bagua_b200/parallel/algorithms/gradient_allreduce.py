@@ -56,12 +56,13 @@ class GradientAllReduceAlgorithm(Algorithm):
 # Checkpointable state of the in-bucket optimizers
 # ---------------------------------------------------------------------------------------------------------------
 _STATE_KEYS = {"sgd": ("master", "momentum_buffer"), "adam": ("master", "exp_avg", "exp_avg_sq"), "lamb": ("master", "exp_avg", "exp_avg_sq"),
-               "lars": ("master", "momentum_buffer")}
+               "lars": ("master", "momentum_buffer"), "lion": ("master", "exp_avg")}
 # what set_hyper of a rule's bucket ops takes, from a parameter group (a LAMB or LARS bucket's two ops take the same)
 _HYPER = {"sgd": lambda g: (float(g["lr"]), float(g["momentum"]), float(g["dampening"]), float(g["weight_decay"]), bool(g["nesterov"])),
           "adam": lambda g: (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]), bool(g["adamw"])),
           "lamb": lambda g: (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"])),
-          "lars": lambda g: (float(g["lr"]), float(g["momentum"]), float(g["weight_decay"]), float(g["trust_coefficient"]))}
+          "lars": lambda g: (float(g["lr"]), float(g["momentum"]), float(g["weight_decay"]), float(g["trust_coefficient"])),
+          "lion": lambda g: (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["weight_decay"]))}
 # the rules whose trust ratio is a norm over a whole parameter: phase A in the bucket program, then per-bucket norms, one
 # per-parameter exchange and the per-bucket update in step()
 _PER_PARAMETER = ("lamb", "lars")
@@ -753,6 +754,29 @@ def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, tru
     return opt
 
 
+class ShardedFusedLion(object):
+    """Marker mix-in: see :func:`make_sharded_fused_lion`."""
+
+
+def make_sharded_fused_lion(params, lr=1e-4, betas=(0.9, 0.99), weight_decay=0.0, max_grad_norm=None, loss_scaling=False, accumulate_grads=False,
+                            ema_decay=None, ema_every=1):
+    """Lion (see :class:`bagua_b200.ops.optim.FusedLion`) on the in-bucket sharded path: each rank keeps fp32 master weights and the
+    one moment ``exp_avg`` for its 1/N slice of every bucket, 4 bytes per element / N less than Adam. The rule is element-wise, so
+    like SGD and Adam the update runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_lion_kernel``),
+    overlapped with the rest of backward. With ``max_grad_norm``, ``loss_scaling`` or ``accumulate_grads`` the bucket kernels only
+    reduce-scatter into the fp32 gradient shard and ``step()`` runs the update (``shard_lion_kernel``); see
+    :func:`make_sharded_fused_sgd`. With one process, or without a peer engine, it behaves like :class:`bagua_b200.ops.optim.FusedLion`."""
+    from ...ops.optim import FusedLion
+
+    class _ShardedFusedLion(_ShardedStateMixin, FusedLion, ShardedFusedLion):
+        _kind = "lion"
+
+    opt = _ShardedFusedLion(params, lr=lr, betas=betas, weight_decay=weight_decay, master_weights=True, zero_grad_in_step=True)
+    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
+    _set_ema(opt, ema_decay, ema_every)
+    return opt
+
+
 class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
     def __init__(self, process_group, optimizer, average: bool = True):
         super().__init__(process_group, hierarchical=False, average=average)
@@ -861,8 +885,9 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         is_adam = isinstance(opt, ShardedFusedAdam)
         is_lamb = isinstance(opt, ShardedFusedLamb)
         is_lars = isinstance(opt, ShardedFusedLars)
+        is_lion = isinstance(opt, ShardedFusedLion)
         per_param = is_lamb or is_lars
-        if eng is None or bucket._slice is None or not (isinstance(opt, ShardedFusedSGD) or is_adam or per_param):
+        if eng is None or bucket._slice is None or not (isinstance(opt, ShardedFusedSGD) or is_adam or per_param or is_lion):
             return super().init_operations(bagua_ddp, bucket)
         bk = opt._bucketing
         group_index = getattr(bucket, "_fused_group", 0)
@@ -933,7 +958,7 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
                 bk.clip = self._clip_state(eng, bagua_ddp, bucket, flat.device, scaled)
             if exchange or per_param:
                 row = (bk.clip if exchange else bk.lamb)["partials"][[b.name for b in bagua_ddp.bagua_buckets].index(bucket.name)]
-            else:   # SGD / Adam accumulating without a norm exchange: partials nobody reads, and an update coefficient of exactly 1
+            else:   # SGD / Adam / Lion accumulating without a norm exchange: partials nobody reads, and an update coefficient of exactly 1
                 row = rec["partials"] = torch.zeros(C.MAX_COMM_BLOCKS, dtype=torch.float64, device=flat.device)
                 if bk.unit is None:
                     bk.unit = torch.ones(1, dtype=torch.float32, device=flat.device)
@@ -945,12 +970,18 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
             coef_ptr = bk.clip["out"][1:].data_ptr() if exchange else (bk.unit.data_ptr() if not per_param else 0)
         if per_param:
             op, moments = self._per_param_ops(eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr, is_lars)
+        elif two_phase and is_lion:
+            op = C.ShardLionOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
+                               use_mc, cfg)
         elif two_phase and is_adam:
             op = C.ShardAdamOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
                                second.data_ptr(), use_mc, cfg)
         elif two_phase:
             op = C.ShardSgdOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
                               use_mc, cfg)
+        elif is_lion:
+            op = C.AllReduceLionOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
+                                   master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
         elif is_adam:
             op = C.AllReduceAdamOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
                                    master.data_ptr(), momentum.data_ptr(), second.data_ptr(), scale, True, use_mc, cfg)
@@ -962,7 +993,7 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         else:
             bucket.backend_bucket.append_op(op)
         bucket._ops_keepalive.append(op)
-        kind = "fused_lamb_" if is_lamb else ("fused_lars_" if is_lars else ("fused_adam_" if is_adam else "fused_sgd_"))
+        kind = "fused_lamb_" if is_lamb else ("fused_lars_" if is_lars else ("fused_lion_" if is_lion else ("fused_adam_" if is_adam else "fused_sgd_")))
         bucket.allreduce_variant = kind + ("accum_" if accum else "") + ("scaled_" if scaled else "") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
         rec["step_ops"] = (op, moments) if per_param else (op,)   # the update op first: state_dict() saves its count
         if scaled:   # the ops obey the exchange's vote and take the step count it keeps on the device
@@ -1057,7 +1088,8 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
 
 class FusedGradientAllReduceAlgorithm(Algorithm):
     """Gradient allreduce whose buckets also apply the optimizer update (see :func:`make_sharded_fused_sgd` /
-    :func:`make_sharded_fused_adam` / :func:`make_sharded_fused_lamb` / :func:`make_sharded_fused_lars`)."""
+    :func:`make_sharded_fused_adam` / :func:`make_sharded_fused_lamb` / :func:`make_sharded_fused_lars` /
+    :func:`make_sharded_fused_lion`)."""
 
     def __init__(self, optimizer, average: bool = True):
         self.optimizer = optimizer

@@ -29,7 +29,7 @@ __all__ = ["GraphedTrainStep", "graph_safe_optimizer"]
 
 def graph_safe_optimizer(opt: torch.optim.Optimizer) -> Optional[str]:
     """``None`` when ``opt`` may run inside a captured graph, else the reason it may not."""
-    from ..ops.optim import FusedAdam, FusedLAMB, FusedLARS, FusedSGD
+    from ..ops.optim import FusedAdam, FusedLAMB, FusedLARS, FusedLion, FusedSGD
 
     if isinstance(opt, FusedSGD):
         return None
@@ -40,6 +40,9 @@ def graph_safe_optimizer(opt: torch.optim.Optimizer) -> Optional[str]:
     if isinstance(opt, FusedLARS):
         return ("FusedLARS cannot be captured: it builds its multi-tensor tables and momentum buffers on the host at the step that "
                 "first sees a parameter and may copy gradients into fresh buffers each step")
+    if isinstance(opt, FusedLion):
+        return ("FusedLion cannot be captured: it builds its multi-tensor tables and moment buffers on the host at the step that first "
+                "sees a parameter and may copy gradients into fresh buffers each step")
     if isinstance(opt, torch.optim.SGD):
         return None
     if all(g.get("capturable", False) for g in opt.param_groups):

@@ -49,7 +49,8 @@ import bagua_b200 as bagua  # noqa: E402
 from bagua_b200 import models  # noqa: E402
 from bagua_b200.contrib import LoadBalancingDistributedSampler  # noqa: E402
 from bagua_b200.parallel.algorithms import Algorithm, q_adam  # noqa: E402
-from bagua_b200.parallel.algorithms.gradient_allreduce import FusedGradientAllReduceAlgorithm, ShardedFusedAdam, make_sharded_fused_adam  # noqa: E402
+from bagua_b200.parallel.algorithms.gradient_allreduce import (FusedGradientAllReduceAlgorithm, ShardedFusedAdam, ShardedFusedLion,  # noqa: E402
+                                                               make_sharded_fused_adam, make_sharded_fused_lion)
 
 _spec = importlib.util.spec_from_file_location("bagua_example_squad_utils", os.path.join(HERE, "squad_utils.py"))
 su = importlib.util.module_from_spec(_spec)
@@ -112,7 +113,9 @@ def parse():
     a("--async-sync-interval", type=int, default=500)
     a("--async-warmup-steps", type=int, default=100)
     a("--fuse-optimizer", action="store_true")
-    a("--fused-shard", action="store_true", help="AdamW inside the bucket kernels (reduce-scatter → update → all-gather)")
+    a("--fused-shard", action="store_true", help="the optimizer inside the bucket kernels (reduce-scatter → update → all-gather)")
+    a("--optimizer", default="adamw", choices=["adamw", "lion"],
+      help="lion: Lion (betas 0.9, 0.99; give it a 3-10x smaller --learning_rate and a larger --weight_decay than AdamW)")
     a("--accumulate-in-shard", action="store_true",
       help="with --fused-shard and --gradient_accumulation_steps > 1: every micro-step communicates and adds its gradient to the fp32 shard")
     a("--load-balance", action="store_true", help="LoadBalancingDistributedSampler keyed on the number of non-pad tokens")
@@ -257,6 +260,14 @@ def make_optimizer(args, model, cuda, world):
         opt = q_adam.QAdamOptimizer(model.parameters(), lr=args.learning_rate, warmup_steps=100, eps=args.adam_epsilon, weight_decay=args.weight_decay)
         return opt, q_adam.QAdamAlgorithm(opt)
     in_shard = args.accumulate_in_shard and args.gradient_accumulation_steps > 1
+    if args.optimizer == "lion":   # the in-bucket Lion also runs without a GPU (all-reduce + FusedLion's CPU update)
+        if args.fused_shard and args.algorithm == "gradient_allreduce":
+            opt = make_sharded_fused_lion(groups, lr=args.learning_rate, max_grad_norm=args.max_grad_norm if args.max_grad_norm > 0 else None,
+                                          loss_scaling=args.dtype == "fp16", accumulate_grads=in_shard)
+            return opt, FusedGradientAllReduceAlgorithm(opt)
+        opt = bagua.ops.FusedLion(groups, lr=args.learning_rate)
+        kw = dict(sync_interval_ms=args.async_sync_interval, warmup_steps=args.async_warmup_steps) if args.algorithm == "async" else {}
+        return opt, Algorithm.init(args.algorithm, **kw)
     # without a GPU the in-shard accumulation runs on the fallback (all-reduce + flat AdamW), which accumulates in the model's dtype
     if args.fused_shard and (cuda or in_shard) and args.algorithm == "gradient_allreduce":
         opt = make_sharded_fused_adam(groups, lr=args.learning_rate, eps=args.adam_epsilon, adamw=True,   # buckets are cut per parameter group
@@ -321,7 +332,7 @@ def train(args, model, tokenizer, dev, rank, world, cuda):
 
         return torch.cuda.nvtx.range(name) if (cuda and args.prof >= 0) else contextlib.nullcontext()
 
-    sharded = isinstance(optimizer, ShardedFusedAdam)
+    sharded = isinstance(optimizer, (ShardedFusedAdam, ShardedFusedLion))
     in_shard = sharded and optimizer.accumulate_grads   # every micro-step communicates; step() consumes the sum in the shard
     grad_norm = None
     # fp16: the scaler hands its device scale to the sharded optimizer, whose step program unscales, votes on overflow and skips
@@ -418,6 +429,8 @@ def main():
     dev = torch.device("cuda", bagua.get_local_rank()) if cuda else torch.device("cpu")
     if args.dtype == "fp16" and not (cuda and args.fused_shard and args.algorithm == "gradient_allreduce"):
         raise SystemExit("--dtype fp16 needs a GPU, --fused-shard and --algorithm gradient_allreduce (loss scaling runs in the in-bucket optimizer)")
+    if args.optimizer == "lion" and args.algorithm == "qadam":
+        raise SystemExit("--optimizer lion does not combine with --algorithm qadam, which brings its own optimizer")
     dtype = {"bf16": torch.bfloat16, "fp16": torch.float16}.get(args.dtype, torch.float32) if cuda else torch.float32
 
     model = build_model(args)

@@ -153,6 +153,15 @@ ema_op = C.EmaOp(*eplan.args(), 1e-4, 0)
 timed("multi_tensor_ema_kernel 32M-element shard", lambda: run(ema_op), n * 12)
 pub = C.ShardPublishOp(comm, b.buf, 0, NB, code, eshard.data_ptr(), False, w.cfg(64))
 timed("shard_publish_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(pub), n * 6)
+# in-bucket Lion on the same bucket: the fused kernel (reads the bucket 2B, master and exp_avg 8B; writes master and exp_avg 8B, the
+# weights 2B and the cleared bucket 2B per element) and phase B (reads shard, master, exp_avg 12B; writes 8B + the weights 2B)
+lion = C.AllReduceLionOp(comm, a.buf, b.buf, 0, 0, NB, code, master.data_ptr(), mom.data_ptr(), 1.0, True, False, w.cfg(32))
+lion.set_hyper(1e-4, 0.9, 0.99, 0.1)
+timed("allreduce_lion_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(lion), n * 22)
+unit = torch.ones(1, device=dev)
+slion = C.ShardLionOp(comm, b.buf, 0, NB, code, shard.data_ptr(), unit.data_ptr(), master.data_ptr(), mom.data_ptr(), False, w.cfg(64))
+slion.set_hyper(1e-4, 0.9, 0.99, 0.1)
+timed("shard_lion_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(slion), n * 22)
 del shard, lpart, npart, gpart, eshard
 
 # single-GPU kernels ------------------------------------------------------------------------------------------------------
@@ -164,7 +173,12 @@ model = torch.empty(P, device=dev, dtype=bf)
 timed("flat_sgd_kernel 138M params (bf16 grads, fp32 master, momentum)", lambda: flat_sgd_(p32, g16, mb, lr=0.01, momentum=0.9, zero_grad=True, model=model, first_step=False), P * 22, iters=3)
 e1, e2 = torch.zeros(P, device=dev), torch.zeros(P, device=dev)
 timed("flat_adam_kernel 138M params", lambda: flat_adam_(p32, g16, e1, e2, lr=1e-3, step=2, adamw=True, weight_decay=0.01, zero_grad=True, model=model), P * 30, iters=3)
-del p32, g16, mb, model, e1, e2
+# multi-tensor Lion over the same arena as one bf16 parameter with an fp32 master: reads the gradient 2B, master and exp_avg 8B; writes
+# the parameter 2B, master and exp_avg 8B and the cleared gradient 2B per element
+lplan = multi_tensor_plan([[model], [g16], [p32], [e1]])
+timed("multi_tensor_lion_kernel<bf16,mixed> 138M params", lambda: C.multi_tensor_lion(*lplan.args(), code, True, 1e-4, 0.9, 0.99, 0.1, True, stream), P * 22,
+      iters=3)
+del p32, g16, mb, model, e1, e2, lplan
 xq = torch.randn(64 * 1024 * 1024, device=dev).to(bf)
 qbuf = quant.compress(xq, 8)
 timed("minmax_uint8_compress 64M bf16, 8 chunks", lambda: quant.compress(xq, 8, out=qbuf), xq.numel() * 5)
