@@ -96,6 +96,9 @@ class MoEPeerContext:
         w [E_local, N, K].  The wgmma GEMM's epilogue stores every 128-row tile straight into the symmetric buffer of the
         rank the tokens came from; the local-layout gather (which opens with the peer barrier) then forms
         out[s] = Σ_k weights[s,k] · row.  Returns (out [S, N], picked [S, k, N])."""
+        from .gemm import _check_grouped_shapes
+
+        _check_grouped_shapes(x, w, bias, names=("x", "w"))
         E_local, _, Kdim = x.shape
         N = w.shape[1]
         K = expert_idx.shape[1]
@@ -172,6 +175,7 @@ class _LinearCombine(torch.autograd.Function):
         w32 = weights.float().contiguous()
         out, picked = pctx.linear_push_gather(x, w, bias, expert_idx, slot_idx, w32, S, C)
         ctx.pctx, ctx.C, ctx.wdtype, ctx.has_bias = pctx, C, weights.dtype, bias is not None
+        ctx.bias_dtype = bias.dtype if bias is not None else None
         ctx.save_for_backward(x, w, expert_idx, slot_idx, w32, picked)
         return out
 
@@ -196,7 +200,7 @@ class _LinearCombine(torch.autograd.Function):
             else:
                 gw = torch.bmm(gy.transpose(1, 2), x)
         if ctx.has_bias and ctx.needs_input_grad[2]:
-            gb = gy.float().sum(dim=1).to(gy.dtype)
+            gb = gy.float().sum(dim=1).to(ctx.bias_dtype)   # summed in fp32, returned in the bias's own dtype
         return gx, gw, gb, grad_w.to(ctx.wdtype), None, None, None, None
 
 

@@ -463,62 +463,6 @@ def test_weight_gate_orders_apply_after_the_trainer_release(C):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# MoE token exchange
-# ---------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("P", [1, 2, 4, 8])
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
-def test_moe_scatter_gather_match_index_oracle(C, P, dtype):
-    w = _world(P)
-    S, K, M, E_local, Cap = 96, 2, 64, 2, 40
-    E = E_local * P
-    es = torch.empty(0, dtype=dtype).element_size()
-    rows_bytes = P * E_local * Cap * M * es
-    buf = w.alloc(rows_bytes)
-    gen = torch.Generator(device="cpu").manual_seed(51)
-    toks, eidx, sidx, wts = [], [], [], []
-    for r in range(P):
-        toks.append(torch.randn(S, M, generator=gen).to(dtype).cuda())
-        e = torch.stack([torch.randperm(E, generator=gen)[:K] for _ in range(S)])          # K distinct experts per token
-        slot = torch.full((S, K), -1, dtype=torch.int64)
-        fill = [0] * E
-        for s in range(S):
-            for k in range(K):
-                ex = int(e[s, k])
-                if fill[ex] < Cap and not (s % 7 == 0 and k == 1):                         # some dropped tokens
-                    slot[s, k] = fill[ex]
-                    fill[ex] += 1
-        eidx.append(e.cuda())
-        sidx.append(slot.cuda())
-        wts.append(torch.rand(S, K, generator=gen).cuda())
-    w.launch_all(lambda r, st: C.moe_scatter(w.comms[r], buf.buf, 0, toks[r].data_ptr(), eidx[r].data_ptr(), sidx[r].data_ptr(), 0, S, K, M, E_local, Cap,
-                                             _code(dtype), 4, st))
-    want = [torch.zeros(P, E_local, Cap, M, dtype=dtype, device="cuda") for _ in range(P)]
-    for r in range(P):
-        for s in range(S):
-            for k in range(K):
-                sl = int(sidx[r][s, k])
-                if sl >= 0:
-                    ex = int(eidx[r][s, k])
-                    want[ex // E_local][r, ex % E_local, sl] = toks[r][s]
-    for o in range(P):
-        got = buf.view(o, dtype, P * E_local * Cap * M).view(P, E_local, Cap, M)
-        assert torch.equal(got, want[o]), f"owner {o}: dispatched rows differ (unfilled slots must read as zeros)"
-    # experts "process" their rows (x2), then every source rank gathers its weighted combination
-    for o in range(P):
-        buf.view(o, dtype, P * E_local * Cap * M).mul_(2)
-    outs = [torch.empty(S, M, dtype=dtype, device="cuda") for _ in range(P)]
-    picked = [torch.empty(S, K, M, dtype=dtype, device="cuda") for _ in range(P)]
-    w.launch_all(lambda r, st: C.moe_gather(w.comms[r], buf.buf, 0, outs[r].data_ptr(), eidx[r].data_ptr(), sidx[r].data_ptr(), wts[r].data_ptr(),
-                                            picked[r].data_ptr(), S, K, M, E_local, Cap, _code(dtype), 4, st, False))
-    for r in range(P):
-        valid = (sidx[r] >= 0).float().unsqueeze(-1)
-        rows = toks[r].float().unsqueeze(1) * 2 * valid                      # [S, K, M]: the processed row of (s, k) or zero
-        ref = (rows * wts[r].unsqueeze(-1)).sum(1)
-        assert (outs[r].float() - ref).abs().max().item() <= (1e-5 if dtype == torch.float32 else 8e-2)
-        torch.testing.assert_close(picked[r].float(), rows.to(dtype).float(), rtol=0, atol=0)
-
-
-# ---------------------------------------------------------------------------------------------------------------------
 # a failed collective is fatal
 # ---------------------------------------------------------------------------------------------------------------------
 def test_a_lonely_collective_times_out_and_poisons_the_communicator(C):
@@ -541,31 +485,3 @@ def test_a_lonely_collective_times_out_and_poisons_the_communicator(C):
     w2.comms[0].abort()
     torch.cuda.synchronize()
     assert w2.comms[0].error_code() == 2
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# grouped GEMM whose epilogue is the MoE combine: every 128-row tile lands in the buffer of the rank that sent those rows
-# ---------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("P", [1, 2, 4])
-def test_grouped_gemm_push_stores_each_source_tile_on_its_owner(C, P):
-    w = _world(P)
-    G, cap, K = 2, 256, 128
-    gen = torch.Generator(device="cpu").manual_seed(60 + P)
-    for N, act in ((256, 0), (384, 1)):                      # BN = 256 and BN = 128 instantiations, plain and GELU epilogue
-        out_bytes = P * G * cap * N * 2
-        buf = w.alloc(out_bytes)
-        A = [(torch.randn(G, P * cap, K, generator=gen) * 0.5).to(torch.bfloat16).cuda() for _ in range(P)]   # rows [source rank][slot]
-        B = [(torch.randn(G, N, K, generator=gen) * 0.5).to(torch.bfloat16).cuda() for _ in range(P)]
-        bias = [torch.randn(G, N, generator=gen).cuda() for _ in range(P)]
-        w.launch_all(lambda r, st: C.grouped_gemm_tn_push(A[r].data_ptr(), B[r].data_ptr(), bias[r].data_ptr(), G, N, K, act, w.comms[r], buf.buf, 0,
-                                                          cap, st))
-        torch.cuda.synchronize()
-        for r in range(P):
-            ref = torch.bmm(A[r].float(), B[r].float().transpose(1, 2)) + bias[r].unsqueeze(1)
-            if act == 1:
-                ref = torch.nn.functional.gelu(ref, approximate="tanh")
-            for s in range(P):                                # owner s holds, at [r][g][slot], what expert g of rank r made of s's rows
-                got = buf.view(s, torch.bfloat16, P * G * cap * N).view(P, G, cap, N)[r].float()
-                want = ref[:, s * cap:(s + 1) * cap]
-                torch.testing.assert_close(got, want, rtol=2e-2, atol=2e-2 * want.abs().max().item())
-    w.check()
