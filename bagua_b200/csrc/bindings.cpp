@@ -50,6 +50,54 @@ void def_stepped(py::class_<Op, CommOp, std::shared_ptr<Op>>& cls) {
     cls.def("set_hyper", [](Op& op, Args... args) { op.set_hyper({args...}); }).def("steps", &Op::steps).def("set_steps", &Op::set_steps)
         .def("set_device_step", &Op::set_device_step, py::arg("vote_ptr"), py::arg("step_ptr"));
 }
+
+template <class...>
+struct Types {};
+
+// A constructor argument that fills a field of a rule struct (kernels.h): a device address becomes the field's pointer type, a count
+// stays an int.
+struct Field {
+    uint64_t addr;
+    template <class T>
+    operator T*() const { return reinterpret_cast<T*>(addr); }
+};
+Field field(uint64_t addr) { return {addr}; }
+int field(int n) { return n; }
+
+// The ops of one in-bucket optimizer rule under their Python names: the fused op (`fused`, when the rule has one) and the phase-B op
+// (`shard`), with def_stepped's methods for the hyper-parameters `Hyper`. Their constructors take the rule struct's fields, of types
+// `State` and named `names`, between the op's own arguments:
+//   fused  (comm, grads, weights, g_off, w_off, bytes, dtype, <state>, scale, zero_grads, use_multimem, cfg)
+//   shard  (comm, weights, w_off, bytes, dtype, shard_ptr, coef_ptr, <state>, use_multimem, cfg); without shard_ptr and coef_ptr for
+//          a rule that reads neither (LAMB).
+template <class Rule, class... Hyper, class... State, class... Names>
+void def_rule_ops(py::module_& m, const char* fused, const char* shard, Types<Hyper...>, Types<State...>, Names... names) {
+    if constexpr (!std::is_same_v<Rule, LambRule> && !std::is_same_v<Rule, LarsRule>) {
+        using Op = FusedUpdateOp<Rule>;
+        def_stepped<Op, Hyper...>(py::class_<Op, CommOp, std::shared_ptr<Op>>(m, fused).def(
+            py::init([](std::shared_ptr<PeerComm> comm, SymmBuf grads, SymmBuf weights, size_t g_off, size_t w_off, size_t bytes, int dtype, State... state,
+                        float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg) {
+                return std::make_shared<Op>(std::move(comm), grads, weights, g_off, w_off, bytes, dtype, Rule{field(state)...}, scale, zero_grads,
+                                            use_multimem, cfg);
+            }),
+            py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), names...,
+            py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg")));
+    }
+    using Op = ShardUpdateOp<Rule>;
+    py::class_<Op, CommOp, std::shared_ptr<Op>> cls(m, shard);
+    auto make = [](std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard_ptr, uint64_t coef_ptr,
+                   State... state, bool use_multimem, LaunchCfg cfg) {
+        return std::make_shared<Op>(std::move(comm), weights, w_off, bytes, dtype, shard_ptr, coef_ptr, Rule{field(state)...}, use_multimem, cfg);
+    };
+    if constexpr (std::is_same_v<Rule, LambRule>)
+        cls.def(py::init([make](std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, State... state, bool use_multimem,
+                                LaunchCfg cfg) { return make(std::move(comm), weights, w_off, bytes, dtype, 0, 0, state..., use_multimem, cfg); }),
+                py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), names..., py::arg("use_multimem"), py::arg("cfg"));
+    else
+        cls.def(py::init(make), py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"),
+                py::arg("coef_ptr"), names..., py::arg("use_multimem"), py::arg("cfg"));
+    def_stepped<Op, Hyper...>(cls);
+}
 }  // namespace
 
 // Entry point for the optional torch extension (csrc/torch_hooks): marks a tensor ready without going through Python.
@@ -231,25 +279,12 @@ PYBIND11_MODULE(_C, m) {
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, uint64_t, uint64_t, size_t, int, float, LaunchCfg>(), py::arg("comm"),
              py::arg("staging"), py::arg("staging_off"), py::arg("slot_bytes"), py::arg("in_ptr"), py::arg("out_ptr"), py::arg("bytes"), py::arg("dtype"),
              py::arg("scale"), py::arg("cfg"));
-    def_stepped<AllReduceSgdOp, float, float, float, float, bool>(
-        py::class_<AllReduceSgdOp, CommOp, std::shared_ptr<AllReduceSgdOp>>(m, "AllReduceSgdOp")
-            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, SymmBuf, size_t, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool,
-                          LaunchCfg>(),
-                 py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"),
-                 py::arg("master_ptr"), py::arg("momentum_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg")));
     py::class_<ReduceScatterOp, CommOp, std::shared_ptr<ReduceScatterOp>>(m, "ReduceScatterOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, float, bool, LaunchCfg>(), py::arg("comm"), py::arg("buf"), py::arg("off"),
              py::arg("bytes"), py::arg("dtype"), py::arg("scale"), py::arg("use_multimem"), py::arg("cfg"));
     py::class_<AllGatherOp, CommOp, std::shared_ptr<AllGatherOp>>(m, "AllGatherOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, bool, LaunchCfg>(), py::arg("comm"), py::arg("buf"), py::arg("off"),
              py::arg("bytes"), py::arg("dtype"), py::arg("use_multimem"), py::arg("cfg"));
-    def_stepped<AllReduceAdamOp, float, float, float, float, float, bool>(
-        py::class_<AllReduceAdamOp, CommOp, std::shared_ptr<AllReduceAdamOp>>(m, "AllReduceAdamOp")
-            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, SymmBuf, size_t, size_t, size_t, int, uint64_t, uint64_t, uint64_t, float, bool, bool,
-                          LaunchCfg>(),
-                 py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"),
-                 py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"),
-                 py::arg("cfg")));
     py::class_<ShardGradOp, CommOp, std::shared_ptr<ShardGradOp>>(m, "ShardGradOp")
         .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool, LaunchCfg, bool>(), py::arg("comm"),
              py::arg("grads"), py::arg("g_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("partials_ptr"), py::arg("scale"),
@@ -269,16 +304,6 @@ PYBIND11_MODULE(_C, m) {
         .def("set_max_norm", &LossScaleNormOp::set_max_norm)
         .def("set_scale_ptr", &LossScaleNormOp::set_scale_ptr)
         .def("calls", &LossScaleNormOp::calls);
-    def_stepped<ShardSgdOp, float, float, float, float, bool>(
-        py::class_<ShardSgdOp, CommOp, std::shared_ptr<ShardSgdOp>>(m, "ShardSgdOp")
-            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(), py::arg("comm"),
-                 py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"), py::arg("master_ptr"),
-                 py::arg("momentum_ptr"), py::arg("use_multimem"), py::arg("cfg")));
-    def_stepped<ShardAdamOp, float, float, float, float, float, bool>(
-        py::class_<ShardAdamOp, CommOp, std::shared_ptr<ShardAdamOp>>(m, "ShardAdamOp")
-            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(),
-                 py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
-                 py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("use_multimem"), py::arg("cfg")));
     def_stepped<LambMomentsOp, float, float, float, float, float>(
         py::class_<LambMomentsOp, CommOp, std::shared_ptr<LambMomentsOp>>(m, "LambMomentsOp")
             .def(py::init<uint64_t, uint64_t, uint64_t, uint64_t, int, int, int, uint64_t, uint64_t>(), py::arg("ptrs"), py::arg("sizes"), py::arg("b2t"),
@@ -288,32 +313,21 @@ PYBIND11_MODULE(_C, m) {
              py::arg("box_off"), py::arg("seg_ptr"), py::arg("seg_nblk"), py::arg("nparams"), py::arg("ratio_ptr"), py::arg("sums_ptr"))
         .def("calls", &LambRatioOp::calls)
         .def_static("box_bytes", &LambRatioOp::box_bytes);
-    def_stepped<ShardLambOp, float, float, float, float, float>(
-        py::class_<ShardLambOp, CommOp, std::shared_ptr<ShardLambOp>>(m, "ShardLambOp")
-            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, int, uint64_t, bool, LaunchCfg>(),
-                 py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("master_ptr"), py::arg("exp_avg_ptr"),
-                 py::arg("exp_avg_sq_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("ratio_ptr"), py::arg("use_multimem"), py::arg("cfg")));
     def_stepped<LarsNormsOp, float, float, float, float>(
         py::class_<LarsNormsOp, CommOp, std::shared_ptr<LarsNormsOp>>(m, "LarsNormsOp")
             .def(py::init<uint64_t, uint64_t, uint64_t, uint64_t, int, int, int, uint64_t, uint64_t>(), py::arg("ptrs"), py::arg("sizes"), py::arg("b2t"),
                  py::arg("b2c"), py::arg("n_tensors"), py::arg("n_blocks"), py::arg("chunk"), py::arg("coef_ptr"), py::arg("partials_ptr")));
-    def_stepped<ShardLarsOp, float, float, float, float>(
-        py::class_<ShardLarsOp, CommOp, std::shared_ptr<ShardLarsOp>>(m, "ShardLarsOp")
-            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, uint64_t, int, uint64_t, bool,
-                          LaunchCfg>(),
-                 py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
-                 py::arg("master_ptr"), py::arg("momentum_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("sums_ptr"), py::arg("use_multimem"),
-                 py::arg("cfg")));
-    def_stepped<AllReduceLionOp, double, double, double, double>(
-        py::class_<AllReduceLionOp, CommOp, std::shared_ptr<AllReduceLionOp>>(m, "AllReduceLionOp")
-            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, SymmBuf, size_t, size_t, size_t, int, uint64_t, uint64_t, float, bool, bool, LaunchCfg>(),
-                 py::arg("comm"), py::arg("grads"), py::arg("weights"), py::arg("g_off"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"),
-                 py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("scale"), py::arg("zero_grads"), py::arg("use_multimem"), py::arg("cfg")));
-    def_stepped<ShardLionOp, double, double, double, double>(
-        py::class_<ShardLionOp, CommOp, std::shared_ptr<ShardLionOp>>(m, "ShardLionOp")
-            .def(py::init<std::shared_ptr<PeerComm>, SymmBuf, size_t, size_t, int, uint64_t, uint64_t, uint64_t, uint64_t, bool, LaunchCfg>(),
-                 py::arg("comm"), py::arg("weights"), py::arg("w_off"), py::arg("bytes"), py::arg("dtype"), py::arg("shard_ptr"), py::arg("coef_ptr"),
-                 py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("use_multimem"), py::arg("cfg")));
+    using Ptr = uint64_t;
+    def_rule_ops<SgdRule>(m, "AllReduceSgdOp", "ShardSgdOp", Types<float, float, float, float, bool>{}, Types<Ptr, Ptr>{}, py::arg("master_ptr"),
+                          py::arg("momentum_ptr"));
+    def_rule_ops<AdamRule>(m, "AllReduceAdamOp", "ShardAdamOp", Types<float, float, float, float, float, bool>{}, Types<Ptr, Ptr, Ptr>{},
+                           py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"));
+    def_rule_ops<LionRule>(m, "AllReduceLionOp", "ShardLionOp", Types<double, double, double, double>{}, Types<Ptr, Ptr>{}, py::arg("master_ptr"),
+                           py::arg("exp_avg_ptr"));
+    def_rule_ops<LambRule>(m, nullptr, "ShardLambOp", Types<float, float, float, float, float>{}, Types<Ptr, Ptr, Ptr, Ptr, int, Ptr>{},
+                           py::arg("master_ptr"), py::arg("exp_avg_ptr"), py::arg("exp_avg_sq_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("ratio_ptr"));
+    def_rule_ops<LarsRule>(m, nullptr, "ShardLarsOp", Types<float, float, float, float>{}, Types<Ptr, Ptr, Ptr, int, Ptr>{}, py::arg("master_ptr"),
+                           py::arg("momentum_ptr"), py::arg("segs_ptr"), py::arg("nsegs"), py::arg("sums_ptr"));
     py::class_<EmaOp, CommOp, std::shared_ptr<EmaOp>>(m, "EmaOp")
         .def(py::init<uint64_t, uint64_t, uint64_t, uint64_t, int, int, int, float, uint64_t>(), py::arg("ptrs"), py::arg("sizes"), py::arg("b2t"),
              py::arg("b2c"), py::arg("n_tensors"), py::arg("n_blocks"), py::arg("chunk"), py::arg("weight"), py::arg("vote_ptr"))

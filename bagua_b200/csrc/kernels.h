@@ -5,6 +5,7 @@
 #include <cmath>
 #include <cstddef>
 #include <cstdint>
+#include <tuple>
 #include <type_traits>
 
 #include "common.h"
@@ -88,28 +89,84 @@ inline LambParams lamb_params(float lr, float beta1, float beta2, float eps, flo
     return LambParams{lr, beta1, beta2, eps, weight_decay, bias_correction(beta1, step), bias_correction(beta2, step)};
 }
 
+// ---- in-bucket optimizer rules (peer_kernels.cu) ---------------------------------------------------------------
+// What an in-bucket optimizer kernel receives of its rule, by value: the fp32 state of the owned shard (shard-local, like the master)
+// and, as an argument of its own, the rule's Params. fields() lists the fields in order, kFused / kShard name the rule's fused and
+// phase-B kernels in messages and op kinds.
+struct SgdRule {
+    static constexpr const char* kFused = "allreduce_sgd";
+    static constexpr const char* kShard = "shard_sgd";
+    using Params = SgdParams;
+    float* master;
+    float* momentum;
+    auto fields() const { return std::tuple(master, momentum); }
+};
+// Params carry the bias corrections of THIS step
+struct AdamRule {
+    static constexpr const char* kFused = "allreduce_adam";
+    static constexpr const char* kShard = "shard_adam";
+    using Params = AdamParams;
+    float* master;
+    float* exp_avg;
+    float* exp_avg_sq;
+    auto fields() const { return std::tuple(master, exp_avg, exp_avg_sq); }
+};
+// g = fl(x·coef) with x the reduced gradient (coef = scale) or the fp32 gradient shard (see lion.cuh)
+struct LionRule {
+    static constexpr const char* kFused = "allreduce_lion";
+    static constexpr const char* kShard = "shard_lion";
+    using Params = LionParams;
+    float* master;
+    float* exp_avg;
+    auto fields() const { return std::tuple(master, exp_avg); }
+};
+// Phase B only: w ← w − lr·r·u on the owned slice, u recomputed from the stage-1 moments, r = ratio[segs[3s+2]] for the elements
+// [segs[3s], segs[3s+1]) of the shard (1 elsewhere, and everywhere when weight_decay == 0).
+struct LambRule {
+    static constexpr const char* kShard = "shard_lamb";
+    using Params = LambParams;
+    float* master;
+    const float* exp_avg;
+    const float* exp_avg_sq;
+    const int32_t* segs;
+    int nsegs;
+    const float* ratio;
+    auto fields() const { return std::tuple(master, exp_avg, exp_avg_sq, segs, nsegs, ratio); }
+};
+// Phase B only: momentum and update of the owned slice with trust = lars_trust(sums of segs[3s+2]) for the elements [segs[3s],
+// segs[3s+1]) (1 in the gaps), g̃ = shard·*coef (coef nullable = 1).
+struct LarsRule {
+    static constexpr const char* kShard = "shard_lars";
+    using Params = LarsParams;
+    float* master;
+    float* momentum;
+    const int32_t* segs;
+    int nsegs;
+    const double* sums;
+    auto fields() const { return std::tuple(master, momentum, segs, nsegs, sums); }
+};
+
 // ---- peer kernels (peer_kernels.cu) ------------------------------------------------------------------------
 void launch_allreduce(const PeerCtx& ctx, const PeerBuf& src, const PeerBuf& dst, size_t src_off, size_t dst_off, size_t bytes,
                       int dtype, float scale, int variant, int nblocks, int nthreads, cudaStream_t stream);
 void launch_allreduce_oneshot(const PeerCtx& ctx, const PeerBuf& staging, size_t staging_off, size_t slot_bytes, const void* in, void* out,
                               size_t bytes, int dtype, float scale, int nblocks, int nthreads, cudaStream_t stream, uint32_t call_parity);
-void launch_allreduce_sgd(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off,
-                          size_t bytes, int dtype, float* master, float* momentum, const SgdParams& hp, float scale,
-                          bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream);
 // Halves of the two-shot schedule (hierarchical all-reduce): in-place reduce of slice `rank` over the group (scaled), and
 // publication of slice `rank` to every peer. Slices are ceil(vecs / world) 16-byte vectors.
 void launch_reduce_scatter(const PeerCtx& ctx, const PeerBuf& buf, size_t off, size_t bytes, int dtype, float scale, bool use_multimem, int nblocks,
                            int nthreads, cudaStream_t stream);
 void launch_all_gather(const PeerCtx& ctx, const PeerBuf& buf, size_t off, size_t bytes, int dtype, bool use_multimem, int nblocks, int nthreads,
                        cudaStream_t stream);
-// Adam / AdamW variant (fp32 master + both moments sharded world ways); hp carries the bias corrections of THIS step.
-void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
-                           float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, float scale, bool zero_grads, bool use_multimem,
-                           int nblocks, int nthreads, cudaStream_t stream);
+// reduce-scatter(grads) → the rule on the owned shard (fp32 master + state sharded world ways) → all-gather of the weights, and the
+// gradient bucket cleared when zero_grads; g = red·scale. Instantiated for SgdRule, AdamRule and LionRule.
+template <class Rule>
+void launch_fused_update(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
+                         const Rule& rule, const typename Rule::Params& hp, float scale, bool zero_grads, bool use_multimem, int nblocks, int nthreads,
+                         cudaStream_t stream);
 // Global-norm clipping of the in-bucket optimizers (see shard_grad_kernel): phase A reduce-scatters a bucket into the fp32 gradient
 // `shard` of the owned slice (scaled) and leaves one fp64 Σx² per CTA in partials[block]; grad_norm sums partials[0..nslots) and
 // *extra (nullable), exchanges the per-rank sums through the symmetric `box` (2·kMaxPeers doubles at box_off) and writes
-// out = {total, coef}; phase B applies SGD / Adam to the shard scaled by *coef and all-gathers the weights. With `accumulate` phase A
+// out = {total, coef}; phase B applies the rule to the shard scaled by *coef and all-gathers the weights. With `accumulate` phase A
 // adds the scaled reduction into the shard (gradient accumulation) and Σx² is the accumulated shard's; preload_shard_grad_accum
 // loads that instantiation for one dtype / world / flavour.
 void launch_shard_grad(const PeerCtx& ctx, const PeerBuf& grads, size_t g_off, size_t bytes, int dtype, float* shard, double* partials, float scale,
@@ -122,44 +179,23 @@ void launch_grad_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, co
 // out = {total = sqrt(S)/scale, coef = (1/scale)·min(max_norm/(total + 1e-6), 1) (max_norm = +inf: no bound), found_inf = !isfinite(S)}
 // and *step += !found_inf, the optimizer's effective step count. The phase-B launchers take that counter as `step` (nullable = the
 // behaviour above): `coef` then addresses {coef, found_inf}; on found_inf the kernel goes straight to its closing barrier, otherwise
-// hp's bias corrections / first_step are rebuilt on the device from t = *step.
+// the rule's bias corrections / first_step are rebuilt on the device from t = *step.
 void launch_loss_scale_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const double* partials, int nslots, const double* extra,
                             const float* scale, float max_norm, uint32_t parity, float* out, uint32_t* step, cudaStream_t stream);
-void launch_shard_sgd(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                      float* master, float* momentum, const SgdParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream,
-                      const uint32_t* step = nullptr);
-void launch_shard_adam(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                       float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, bool use_multimem, int nblocks, int nthreads,
-                       cudaStream_t stream, const uint32_t* step = nullptr);
-// In-bucket LAMB. The moments of every shard run as launch_multi_tensor_lamb_stage1 over the shard's segments (one parameter ∩ the
-// owned slice each). lamb_ratio: parameter t's local {Σw², Σu²} is the fixed-order sum of the seg_nblk[t] stage-1 partials at
-// seg_ptr[t] (0 blocks: no segment on this rank); the per-rank pairs are exchanged through the symmetric `box`
-// (2 halves · kMaxPeers · nparams double2 at box_off, half = parity) and summed in rank order → ratio[t] (fp32, identical bits on
-// every rank) and sums[t]. shard_lamb: w ← w − lr·r·u on the owned slice, r = ratio[segs[3s+2]] for the elements
-// [segs[3s], segs[3s+1]) of the shard (1 elsewhere, and everywhere when weight_decay == 0), then the weights are all-gathered.
-// `vote` = {coef, found_inf} and `step` as for launch_shard_sgd (both null without loss scaling).
+// Phase B of every rule: the update of the owned shard from the fp32 gradient `shard` (LAMB: from the master; shard unused) with the
+// coefficient *coef (LARS: nullable = 1; LAMB: none), then the all-gather of the weights and a closing barrier. With `step` (loss
+// scaling, see above) coef addresses {coef, found_inf}, which LAMB takes as its vote alone.
+template <class Rule>
+void launch_shard_update(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                         const Rule& rule, const typename Rule::Params& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream,
+                         const uint32_t* step = nullptr);
+// In-bucket LAMB and LARS. The moments (LAMB) or the norms (LARS) of every shard run as launch_multi_tensor_{lamb,lars}_stage1 over
+// the shard's segments (one parameter ∩ the owned slice each). lamb_ratio: parameter t's local pair ({Σw², Σu²} or {Σw², Σg̃²}) is the
+// fixed-order sum of the seg_nblk[t] stage-1 partials at seg_ptr[t] (0 blocks: no segment on this rank); the per-rank pairs are
+// exchanged through the symmetric `box` (2 halves · kMaxPeers · nparams double2 at box_off, half = parity) and summed in rank order →
+// ratio[t] (fp32, identical bits on every rank; unused by LARS) and sums[2t], sums[2t+1]. launch_shard_update then applies the rule.
 void launch_lamb_ratio(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const uint64_t* seg_ptr, const int32_t* seg_nblk, int nparams,
                        uint32_t parity, float* ratio, double* sums, cudaStream_t stream);
-void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, float* master, const float* exp_avg,
-                       const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, const LambParams& hp, bool use_multimem,
-                       int nblocks, int nthreads, cudaStream_t stream, const float* vote = nullptr, const uint32_t* step = nullptr);
-// In-bucket LARS, the same program as LAMB: launch_multi_tensor_lars_stage1 over the shard's segments ([master, gradient shard]
-// lists) leaves fp64 {Σw², Σg̃²} per block, launch_lamb_ratio exchanges them per parameter (its `ratio` output goes unused) into
-// sums[2t], sums[2t+1], and shard_lars applies the update to the owned slice with trust = lars_trust(sums of segs[3s+2]) for the
-// elements [segs[3s], segs[3s+1]) (1 in the gaps), g̃ = shard·*coef (coef nullable = 1), then all-gathers the weights. `vote`: coef
-// addresses {coef, found_inf} and a found_inf step goes straight to the closing barrier.
-void launch_shard_lars(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                       float* master, float* momentum, const int32_t* segs, int nsegs, const double* sums, const LarsParams& hp, bool use_multimem,
-                       int nblocks, int nthreads, cudaStream_t stream, bool vote = false);
-// In-bucket Lion (lion.cuh). allreduce_lion: the walk of launch_allreduce_adam with g = fl(red·scale), the fp32 master and exp_avg
-// of the owned shard. shard_lion: phase B over the fp32 gradient shard with g = fl(shard·*coef); with `vote` coef addresses
-// {coef, found_inf} and a found_inf step touches no state and only takes the closing barrier.
-void launch_allreduce_lion(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
-                           float* master, float* exp_avg, const LionParams& hp, float scale, bool zero_grads, bool use_multimem, int nblocks, int nthreads,
-                           cudaStream_t stream);
-void launch_shard_lion(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                       float* master, float* exp_avg, const LionParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream,
-                       bool vote = false);
 // Weight EMA of the in-bucket optimizers: publishes the fp32 shard `src` (the owned slice, shard-local like the master) rounded with
 // Vec16<T>::pack into every rank's copy of the weights, between an opening and a closing barrier. preload_shard_publish loads the
 // instantiation for one dtype / world / flavour.

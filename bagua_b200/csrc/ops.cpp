@@ -121,14 +121,6 @@ void AllReduceOneShotOp::run(Bucket&, StreamHandle stream, int) {
                              bytes_, dtype_, scale_, cfg_.nblocks, cfg_.nthreads, S(stream), comm_->next_oneshot_parity());
 }
 
-void AllReduceSgdOp::run(Bucket&, StreamHandle stream, int) {
-    comm_->check_fatal("allreduce_sgd");
-    if (dev_step()) throw std::runtime_error("bagua: allreduce_sgd updates during backward and cannot take a device-side step count");
-    launch_allreduce_sgd(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_),
-                         reinterpret_cast<float*>(momentum_), params(), scale_, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
-    steps_++;
-}
-
 void ReduceScatterOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("reduce_scatter");
     launch_reduce_scatter(comm_->ctx(), buf_.buf, off_, bytes_, dtype_, scale_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
@@ -137,15 +129,6 @@ void ReduceScatterOp::run(Bucket&, StreamHandle stream, int) {
 void AllGatherOp::run(Bucket&, StreamHandle stream, int) {
     comm_->check_fatal("all_gather");
     launch_all_gather(comm_->ctx(), buf_.buf, off_, bytes_, dtype_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
-}
-
-void AllReduceAdamOp::run(Bucket&, StreamHandle stream, int) {
-    comm_->check_fatal("allreduce_adam");
-    if (dev_step()) throw std::runtime_error("bagua: allreduce_adam updates during backward and cannot take a device-side step count");
-    launch_allreduce_adam(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_),
-                          reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), params(), scale_, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads,
-                          S(stream));
-    steps_++;
 }
 
 ShardGradOp::ShardGradOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, size_t g_off, size_t bytes, int dtype, uint64_t shard, uint64_t partials,
@@ -180,22 +163,6 @@ void LossScaleNormOp::run(Bucket&, StreamHandle stream, int) {
     calls_++;
 }
 
-void ShardSgdOp::run(Bucket&, StreamHandle stream, int) {
-    comm_->check_fatal("shard_sgd");
-    launch_shard_sgd(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), coef_or_vote(coef_),
-                     reinterpret_cast<float*>(master_), reinterpret_cast<float*>(momentum_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream),
-                     dev_step());
-    steps_++;
-}
-
-void ShardAdamOp::run(Bucket&, StreamHandle stream, int) {
-    comm_->check_fatal("shard_adam");
-    launch_shard_adam(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), coef_or_vote(coef_),
-                      reinterpret_cast<float*>(master_), reinterpret_cast<float*>(m1_), reinterpret_cast<float*>(m2_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads,
-                      S(stream), dev_step());
-    steps_++;
-}
-
 void LambMomentsOp::run(Bucket&, StreamHandle stream, int) {
     launch_multi_tensor_lamb_stage1(desc_, F32, false, params(), coef_or_vote(coef_), reinterpret_cast<double*>(partials_), false, S(stream), dev_step());
     steps_++;
@@ -208,42 +175,35 @@ void LambRatioOp::run(Bucket&, StreamHandle stream, int) {
     calls_++;
 }
 
-void ShardLambOp::run(Bucket&, StreamHandle stream, int) {
-    comm_->check_fatal("shard_lamb");
-    launch_shard_lamb(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_), reinterpret_cast<const float*>(m1_),
-                      reinterpret_cast<const float*>(m2_), reinterpret_cast<const int32_t*>(segs_), nsegs_, reinterpret_cast<const float*>(ratio_), params(), use_mc_,
-                      cfg_.nblocks, cfg_.nthreads, S(stream), vote(), dev_step());
-    steps_++;
-}
-
 void LarsNormsOp::run(Bucket&, StreamHandle stream, int) {
     launch_multi_tensor_lars_stage1(desc_, F32, false, coef_or_vote(coef_), reinterpret_cast<double*>(partials_), S(stream), vote() != nullptr);
     steps_++;
 }
 
-void ShardLarsOp::run(Bucket&, StreamHandle stream, int) {
-    comm_->check_fatal("shard_lars");
-    launch_shard_lars(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), coef_or_vote(coef_),
-                      reinterpret_cast<float*>(master_), reinterpret_cast<float*>(momentum_), reinterpret_cast<const int32_t*>(segs_), nsegs_,
-                      reinterpret_cast<const double*>(sums_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream), vote() != nullptr);
-    steps_++;
+template <class Rule>
+void FusedUpdateOp<Rule>::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal(Rule::kFused);
+    if (this->vote()) throw std::runtime_error(std::string("bagua: ") + Rule::kFused + " updates during backward and cannot obey a device-side vote or step count");
+    launch_fused_update(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, rule_, this->params(), scale_, zero_grads_, use_mc_,
+                        cfg_.nblocks, cfg_.nthreads, S(stream));
+    this->steps_++;
 }
+template class FusedUpdateOp<SgdRule>;
+template class FusedUpdateOp<AdamRule>;
+template class FusedUpdateOp<LionRule>;
 
-void AllReduceLionOp::run(Bucket&, StreamHandle stream, int) {
-    comm_->check_fatal("allreduce_lion");
-    if (vote()) throw std::runtime_error("bagua: allreduce_lion updates during backward and cannot obey a device-side vote");
-    launch_allreduce_lion(comm_->ctx(), grads_.buf, weights_.buf, g_off_, w_off_, bytes_, dtype_, reinterpret_cast<float*>(master_),
-                          reinterpret_cast<float*>(exp_avg_), params(), scale_, zero_grads_, use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream));
-    steps_++;
+template <class Rule>
+void ShardUpdateOp<Rule>::run(Bucket&, StreamHandle stream, int) {
+    comm_->check_fatal(Rule::kShard);
+    launch_shard_update(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), this->coef_or_vote(coef_), rule_,
+                        this->params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream), this->dev_step());
+    this->steps_++;
 }
-
-void ShardLionOp::run(Bucket&, StreamHandle stream, int) {
-    comm_->check_fatal("shard_lion");
-    launch_shard_lion(comm_->ctx(), weights_.buf, w_off_, bytes_, dtype_, reinterpret_cast<const float*>(shard_), coef_or_vote(coef_),
-                      reinterpret_cast<float*>(master_), reinterpret_cast<float*>(exp_avg_), params(), use_mc_, cfg_.nblocks, cfg_.nthreads, S(stream),
-                      vote() != nullptr);
-    steps_++;
-}
+template class ShardUpdateOp<SgdRule>;
+template class ShardUpdateOp<AdamRule>;
+template class ShardUpdateOp<LionRule>;
+template class ShardUpdateOp<LambRule>;
+template class ShardUpdateOp<LarsRule>;
 
 void EmaOp::run(Bucket&, StreamHandle stream, int) { launch_multi_tensor_ema(desc_, weight(), reinterpret_cast<const float*>(vote_), S(stream)); }
 

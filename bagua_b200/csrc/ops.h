@@ -181,27 +181,60 @@ private:
     std::mutex mu_;
 };
 
-// reduce-scatter(grads) → SGD on the owned shard → all-gather(weights), one kernel per bucket.
-class AllReduceSgdOp final : public SteppedOp<SgdHyper> {
+// The host side of each in-bucket optimizer rule (kernels.h): its hyper-parameters, and whether its kernel arguments are the same at
+// every launch that follows `steps` earlier ones.
+template <class Rule>
+struct RuleHost;
+template <>
+struct RuleHost<SgdRule> {
+    using Hyper = SgdHyper;
+    static bool step_invariant(uint64_t steps) { return steps > 0; }  // only the very first launch differs (momentum initialisation)
+};
+template <>
+struct RuleHost<AdamRule> {
+    using Hyper = AdamHyper;
+    static bool step_invariant(uint64_t) { return false; }  // bias corrections are passed by value
+};
+template <>
+struct RuleHost<LambRule> {
+    using Hyper = LambHyper;
+    static bool step_invariant(uint64_t) { return false; }  // bias corrections are passed by value
+};
+template <>
+struct RuleHost<LarsRule> {
+    using Hyper = LarsHyper;
+    static bool step_invariant(uint64_t) { return true; }
+};
+template <>
+struct RuleHost<LionRule> {
+    using Hyper = LionHyper;
+    static bool step_invariant(uint64_t) { return true; }
+};
+
+// reduce-scatter(grads) → the rule on the owned shard → all-gather(weights), one kernel per bucket, during backward (SGD, Adam, Lion).
+// `rule` holds the rule's state pointers; each run passes the parameters of its launch.
+template <class Rule>
+class FusedUpdateOp final : public SteppedOp<typename RuleHost<Rule>::Hyper> {
 public:
-    AllReduceSgdOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, SymmBuf weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
-                   uint64_t master, uint64_t momentum, float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), grads_(grads), weights_(weights), g_off_(g_off), w_off_(w_off), bytes_(bytes), dtype_(dtype),
-          master_(master), momentum_(momentum), scale_(scale), zero_grads_(zero_grads), use_mc_(use_multimem), cfg_(cfg) {}
-    const char* kind() const override { return "allreduce_sgd"; }
+    FusedUpdateOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, SymmBuf weights, size_t g_off, size_t w_off, size_t bytes, int dtype, Rule rule,
+                  float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), grads_(grads), weights_(weights), g_off_(g_off), w_off_(w_off), bytes_(bytes), dtype_(dtype), rule_(rule),
+          scale_(scale), zero_grads_(zero_grads), use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return Rule::kFused; }
     void run(Bucket&, StreamHandle stream, int device) override;
-    bool step_invariant() const override { return steps_ > 0; }  // only the very first launch differs (momentum initialisation)
+    bool step_invariant() const override { return RuleHost<Rule>::step_invariant(this->steps_); }
 
 private:
     std::shared_ptr<PeerComm> comm_;
     SymmBuf grads_, weights_;
     size_t g_off_, w_off_, bytes_;
     int dtype_;
-    uint64_t master_, momentum_;
+    Rule rule_;
     const float scale_;
     bool zero_grads_, use_mc_;
     LaunchCfg cfg_;
 };
+
 
 // Intra-node halves of a hierarchical all-reduce (see reduce_scatter_kernel): ReduceScatterOp, then a callback op that
 // all-reduces slice `rank` between nodes, then AllGatherOp.
@@ -238,27 +271,6 @@ private:
     LaunchCfg cfg_;
 };
 
-// The Adam / AdamW flavour of the fused bucket op; the step counter (bias correction) advances with every launch.
-class AllReduceAdamOp final : public SteppedOp<AdamHyper> {
-public:
-    AllReduceAdamOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, SymmBuf weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
-                    uint64_t master, uint64_t exp_avg, uint64_t exp_avg_sq, float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), grads_(grads), weights_(weights), g_off_(g_off), w_off_(w_off), bytes_(bytes), dtype_(dtype),
-          master_(master), m1_(exp_avg), m2_(exp_avg_sq), scale_(scale), zero_grads_(zero_grads), use_mc_(use_multimem), cfg_(cfg) {}
-    const char* kind() const override { return "allreduce_adam"; }
-    void run(Bucket&, StreamHandle stream, int device) override;
-    bool step_invariant() const override { return false; }  // bias corrections are passed by value
-
-private:
-    std::shared_ptr<PeerComm> comm_;
-    SymmBuf grads_, weights_;
-    size_t g_off_, w_off_, bytes_;
-    int dtype_;
-    uint64_t master_, m1_, m2_;
-    const float scale_;
-    bool zero_grads_, use_mc_;
-    LaunchCfg cfg_;
-};
 
 // Global-norm clipping of the in-bucket optimizers (see shard_grad_kernel). Phase A, in the bucket program: reduce-scatter of the
 // gradients into the fp32 shard of the owned slice, per-CTA fp64 Σx² into `partials` (kMaxCommBlocks doubles), bucket cleared.
@@ -341,51 +353,34 @@ private:
     uint64_t calls_ = 0;
 };
 
-// Phase B: SGD on the owned shard with the gradient shard·coef, all-gather of the weights. Carries the step counter like
-// AllReduceSgdOp (checkpoints see the same interface).
-class ShardSgdOp final : public SteppedOp<SgdHyper> {
+// Phase B of every rule, run from step(): the rule on the owned shard from the gradient shard·coef, all-gather of the weights (see
+// shard_update_kernel). LAMB reads the master instead and no coefficient: its shard and coef are 0. With set_device_step the coef is
+// the vote's {coef, found_inf}. Carries the step counter like the fused op (checkpoints see the same interface).
+template <class Rule>
+class ShardUpdateOp final : public SteppedOp<typename RuleHost<Rule>::Hyper> {
 public:
-    ShardSgdOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
-               uint64_t momentum, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), master_(master),
-          momentum_(momentum), use_mc_(use_multimem), cfg_(cfg) {}
-    const char* kind() const override { return "shard_sgd"; }
+    ShardUpdateOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, Rule rule,
+                  bool use_multimem, LaunchCfg cfg)
+        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), rule_(rule),
+          use_mc_(use_multimem), cfg_(cfg) {}
+    const char* kind() const override { return Rule::kShard; }
     void run(Bucket&, StreamHandle stream, int device) override;
-    bool step_invariant() const override { return steps_ > 0; }
+    bool step_invariant() const override { return RuleHost<Rule>::step_invariant(this->steps_); }
 
 private:
     std::shared_ptr<PeerComm> comm_;
     SymmBuf weights_;
     size_t w_off_, bytes_;
     int dtype_;
-    uint64_t shard_, coef_, master_, momentum_;
-    bool use_mc_;
-    LaunchCfg cfg_;
-};
-
-class ShardAdamOp final : public SteppedOp<AdamHyper> {
-public:
-    ShardAdamOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
-                uint64_t exp_avg, uint64_t exp_avg_sq, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), master_(master),
-          m1_(exp_avg), m2_(exp_avg_sq), use_mc_(use_multimem), cfg_(cfg) {}
-    const char* kind() const override { return "shard_adam"; }
-    void run(Bucket&, StreamHandle stream, int device) override;
-    bool step_invariant() const override { return false; }
-
-private:
-    std::shared_ptr<PeerComm> comm_;
-    SymmBuf weights_;
-    size_t w_off_, bytes_;
-    int dtype_;
-    uint64_t shard_, coef_, master_, m1_, m2_;
+    uint64_t shard_, coef_;
+    Rule rule_;
     bool use_mc_;
     LaunchCfg cfg_;
 };
 
 // In-bucket LAMB, run from step() after phase A (ShardGradOp): LambMomentsOp per bucket (the multi-tensor stage-1 kernel over the
 // shard's segment table: fp32 master / gradient shard·*coef / moments, fp64 {Σw², Σu²} per block into `partials`), LambRatioOp once
-// per step (the per-parameter exchange), ShardLambOp per bucket (apply + all-gather + barrier). The moments and apply ops carry the
+// per step (the per-parameter exchange), ShardUpdateOp<LambRule> per bucket (apply + all-gather + barrier). The moments and apply ops carry the
 // step count (bias corrections) and advance together.
 class LambMomentsOp final : public SteppedOp<LambHyper> {
 public:
@@ -422,31 +417,9 @@ private:
     uint64_t calls_ = 0;
 };
 
-class ShardLambOp final : public SteppedOp<LambHyper> {
-public:
-    ShardLambOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t master, uint64_t exp_avg, uint64_t exp_avg_sq,
-                uint64_t segs, int nsegs, uint64_t ratio, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), master_(master), m1_(exp_avg), m2_(exp_avg_sq), segs_(segs),
-          nsegs_(nsegs), ratio_(ratio), use_mc_(use_multimem), cfg_(cfg) {}
-    const char* kind() const override { return "shard_lamb"; }
-    void run(Bucket&, StreamHandle stream, int device) override;
-    bool step_invariant() const override { return false; }
-
-private:
-    std::shared_ptr<PeerComm> comm_;
-    SymmBuf weights_;
-    size_t w_off_, bytes_;
-    int dtype_;
-    uint64_t master_, m1_, m2_, segs_;
-    int nsegs_;
-    uint64_t ratio_;
-    bool use_mc_;
-    LaunchCfg cfg_;
-};
-
 // In-bucket LARS, run from step() after phase A like LAMB: LarsNormsOp per bucket (the multi-tensor LARS stage 1 over the shard's
 // segment table, lists [fp32 master, gradient shard]: fp64 {Σw², Σg̃²} per block into `partials`, g̃ = shard·*coef), the LAMB
-// ratio exchange (LambRatioOp) once per step for the per-parameter global sums, ShardLarsOp per bucket (momentum + apply from the
+// ratio exchange (LambRatioOp) once per step for the per-parameter global sums, ShardUpdateOp<LarsRule> per bucket (momentum + apply from the
 // exchanged sums, all-gather, barrier). The rule has no step-dependent parameter; both ops count their launches for checkpoints.
 class LarsNormsOp final : public SteppedOp<LarsHyper> {
 public:
@@ -460,69 +433,6 @@ public:
 private:
     TensorListDesc desc_;
     uint64_t coef_, partials_;
-};
-
-class ShardLarsOp final : public SteppedOp<LarsHyper> {
-public:
-    ShardLarsOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
-                uint64_t momentum, uint64_t segs, int nsegs, uint64_t sums, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), master_(master),
-          momentum_(momentum), segs_(segs), nsegs_(nsegs), sums_(sums), use_mc_(use_multimem), cfg_(cfg) {}
-    const char* kind() const override { return "shard_lars"; }
-    void run(Bucket&, StreamHandle stream, int device) override;
-
-private:
-    std::shared_ptr<PeerComm> comm_;
-    SymmBuf weights_;
-    size_t w_off_, bytes_;
-    int dtype_;
-    uint64_t shard_, coef_, master_, momentum_, segs_;
-    int nsegs_;
-    uint64_t sums_;
-    bool use_mc_;
-    LaunchCfg cfg_;
-};
-
-// In-bucket Lion. AllReduceLionOp is the Lion flavour of the fused bucket op (update during backward); ShardLionOp is phase B of the
-// two-phase program (after ShardGradOp), the gradient shard·*coef. Lion's kernel arguments hold only the hyper-parameters, which do
-// not depend on the step, so both ops are step-invariant; they count their launches for checkpoints like every optimizer op.
-class AllReduceLionOp final : public SteppedOp<LionHyper> {
-public:
-    AllReduceLionOp(std::shared_ptr<PeerComm> comm, SymmBuf grads, SymmBuf weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
-                    uint64_t master, uint64_t exp_avg, float scale, bool zero_grads, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), grads_(grads), weights_(weights), g_off_(g_off), w_off_(w_off), bytes_(bytes), dtype_(dtype),
-          master_(master), exp_avg_(exp_avg), scale_(scale), zero_grads_(zero_grads), use_mc_(use_multimem), cfg_(cfg) {}
-    const char* kind() const override { return "allreduce_lion"; }
-    void run(Bucket&, StreamHandle stream, int device) override;
-
-private:
-    std::shared_ptr<PeerComm> comm_;
-    SymmBuf grads_, weights_;
-    size_t g_off_, w_off_, bytes_;
-    int dtype_;
-    uint64_t master_, exp_avg_;
-    const float scale_;
-    bool zero_grads_, use_mc_;
-    LaunchCfg cfg_;
-};
-
-class ShardLionOp final : public SteppedOp<LionHyper> {
-public:
-    ShardLionOp(std::shared_ptr<PeerComm> comm, SymmBuf weights, size_t w_off, size_t bytes, int dtype, uint64_t shard, uint64_t coef, uint64_t master,
-                uint64_t exp_avg, bool use_multimem, LaunchCfg cfg)
-        : comm_(std::move(comm)), weights_(weights), w_off_(w_off), bytes_(bytes), dtype_(dtype), shard_(shard), coef_(coef), master_(master),
-          exp_avg_(exp_avg), use_mc_(use_multimem), cfg_(cfg) {}
-    const char* kind() const override { return "shard_lion"; }
-    void run(Bucket&, StreamHandle stream, int device) override;
-
-private:
-    std::shared_ptr<PeerComm> comm_;
-    SymmBuf weights_;
-    size_t w_off_, bytes_;
-    int dtype_;
-    uint64_t shard_, coef_, master_, exp_avg_;
-    bool use_mc_;
-    LaunchCfg cfg_;
 };
 
 // Weight EMA of the in-bucket optimizers. EmaOp is local: one multi-tensor launch of e ← e + w·(m − e) over the table's

@@ -236,89 +236,240 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_kernel(PeerCtx ctx, Pee
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// The optimizer update of one 16-byte vector of the owned shard (N lanes at index j·N of the fp32 state), shared by the in-bucket
-// kernels below and by the clipped two-phase kernels further down: g[k]·scale is the gradient the update sees. w receives the new
-// fp32 weights, which the caller publishes.
+// The in-bucket optimizer rules, device side: Update<R> is the rule struct R of kernels.h (fp32 state of the owned shard, shard-local)
+// with what the two kernels below need of it and of its parameters hp (R::Params). The kernels take R's fields and hp as kernel
+// arguments of their own and build the rule inside: scalar pointer arguments are known to address global memory, and a struct
+// argument's 8-byte alignment would let the compiler pair the loads of hp's fields, so either form compiles to other machine code.
+//   setup(hp)         per-thread values, built once before the walk (Local; empty for most rules)
+//   at_step(hp, t)    rebuilds the step-dependent fields of hp from the device step count t (loss scaling)
+//   source(shard)     what the phase-B walk reads: the fp32 gradient shard, or the master for LAMB
+//   coef(c)           the gradient coefficient of phase B
+//   update<N>(...)    one 16-byte vector of the owned shard (N lanes at index j·N of the fp32 state): g[k]·scale is the gradient the
+//                     update sees; w receives the new fp32 weights, which the caller publishes.
 // ---------------------------------------------------------------------------------------------------------
-template <int N>
-__device__ __forceinline__ void sgd_update(float* master, float* momentum_buf, size_t j, const float* g, float scale, const SgdParams& hp, float* w) {
-    float m[N];
-    float4* mp = reinterpret_cast<float4*>(master + j * N);
-    float4* mo = reinterpret_cast<float4*>(momentum_buf + j * N);
+template <class R>
+struct Update;
+
+template <>
+struct Update<SgdRule> : SgdRule {
+    struct Local {};
+    __device__ __forceinline__ static Local setup(const Params&) { return {}; }
+    __device__ __forceinline__ static void at_step(Params& hp, uint32_t t) { hp.first_step = t == 1u ? 1 : 0; }
+    __device__ __forceinline__ const float* source(const float* shard) const { return shard; }
+    __device__ __forceinline__ float coef(const float* c) const { return *c; }
+    template <int N>
+    __device__ __forceinline__ void update(Local&, const Params& hp, size_t j, const float* g, float scale, float* w) const {
+        float m[N];
+        float4* mp = reinterpret_cast<float4*>(master + j * N);
+        float4* mo = reinterpret_cast<float4*>(momentum + j * N);
 #pragma unroll
-    for (int q = 0; q < N / 4; ++q) {
-        float4 a = mp[q];
-        w[4 * q] = a.x, w[4 * q + 1] = a.y, w[4 * q + 2] = a.z, w[4 * q + 3] = a.w;
-        if (hp.momentum != 0.f) {
-            float4 bb = mo[q];
-            m[4 * q] = bb.x, m[4 * q + 1] = bb.y, m[4 * q + 2] = bb.z, m[4 * q + 3] = bb.w;
+        for (int q = 0; q < N / 4; ++q) {
+            float4 a = mp[q];
+            w[4 * q] = a.x, w[4 * q + 1] = a.y, w[4 * q + 2] = a.z, w[4 * q + 3] = a.w;
+            if (hp.momentum != 0.f) {
+                float4 bb = mo[q];
+                m[4 * q] = bb.x, m[4 * q + 1] = bb.y, m[4 * q + 2] = bb.z, m[4 * q + 3] = bb.w;
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < N; ++k) {
+            float d = g[k] * scale + hp.weight_decay * w[k];
+            if (hp.momentum != 0.f) {
+                m[k] = hp.first_step ? d : hp.momentum * m[k] + (1.f - hp.dampening) * d;
+                d = hp.nesterov ? d + hp.momentum * m[k] : m[k];
+            }
+            w[k] -= hp.lr * d;
+        }
+#pragma unroll
+        for (int q = 0; q < N / 4; ++q) {
+            mp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+            if (hp.momentum != 0.f) mo[q] = make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]);
         }
     }
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-        float d = g[k] * scale + hp.weight_decay * w[k];
-        if (hp.momentum != 0.f) {
-            m[k] = hp.first_step ? d : hp.momentum * m[k] + (1.f - hp.dampening) * d;
-            d = hp.nesterov ? d + hp.momentum * m[k] : m[k];
-        }
-        w[k] -= hp.lr * d;
-    }
-#pragma unroll
-    for (int q = 0; q < N / 4; ++q) {
-        mp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-        if (hp.momentum != 0.f) mo[q] = make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]);
-    }
-}
+};
 
 // Adam / AdamW, update rule identical to flat_adam_kernel (multi_tensor.cu) / torch.optim.Adam[W]; inv_bc1 = 1/(1−β1^t),
 // inv_sqrt_bc2 = 1/sqrt(1−β2^t).
-template <int N>
-__device__ __forceinline__ void adam_update(float* master, float* exp_avg, float* exp_avg_sq, size_t j, const float* g, float scale, const AdamParams& hp,
-                                            float inv_bc1, float inv_sqrt_bc2, float* w) {
-    float4* wp = reinterpret_cast<float4*>(master + j * N);
-    float4* ap = reinterpret_cast<float4*>(exp_avg + j * N);
-    float4* bp = reinterpret_cast<float4*>(exp_avg_sq + j * N);
-#pragma unroll
-    for (int q = 0; q < N / 4; ++q) {
-        float4 ww = wp[q], aa = ap[q], bb = bp[q];
-        float wv[4] = {ww.x, ww.y, ww.z, ww.w}, av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            float gg = g[4 * q + k] * scale;
-            if (hp.adamw)
-                wv[k] *= (1.f - hp.lr * hp.weight_decay);
-            else
-                gg += hp.weight_decay * wv[k];
-            av[k] = hp.beta1 * av[k] + (1.f - hp.beta1) * gg;
-            bv[k] = hp.beta2 * bv[k] + (1.f - hp.beta2) * gg * gg;
-            const float denom = sqrtf(bv[k]) * inv_sqrt_bc2 + hp.eps;
-            wv[k] -= (hp.lr * inv_bc1) * (av[k] / denom);
-            w[4 * q + k] = wv[k];
-        }
-        wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
-        ap[q] = make_float4(av[0], av[1], av[2], av[3]);
-        bp[q] = make_float4(bv[0], bv[1], bv[2], bv[3]);
+template <>
+struct Update<AdamRule> : AdamRule {
+    struct Local {
+        float inv_bc1, inv_sqrt_bc2;
+    };
+    __device__ __forceinline__ static Local setup(const Params& hp) { return {1.f / hp.bias_correction1, rsqrtf(hp.bias_correction2)}; }
+    __device__ __forceinline__ static void at_step(Params& hp, uint32_t t) {
+        hp.bias_correction1 = bias_correction(hp.beta1, t);
+        hp.bias_correction2 = bias_correction(hp.beta2, t);
     }
+    __device__ __forceinline__ const float* source(const float* shard) const { return shard; }
+    __device__ __forceinline__ float coef(const float* c) const { return *c; }
+    template <int N>
+    __device__ __forceinline__ void update(Local& l, const Params& hp, size_t j, const float* g, float scale, float* w) const {
+        float4* wp = reinterpret_cast<float4*>(master + j * N);
+        float4* ap = reinterpret_cast<float4*>(exp_avg + j * N);
+        float4* bp = reinterpret_cast<float4*>(exp_avg_sq + j * N);
+#pragma unroll
+        for (int q = 0; q < N / 4; ++q) {
+            float4 ww = wp[q], aa = ap[q], bb = bp[q];
+            float wv[4] = {ww.x, ww.y, ww.z, ww.w}, av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                float gg = g[4 * q + k] * scale;
+                if (hp.adamw)
+                    wv[k] *= (1.f - hp.lr * hp.weight_decay);
+                else
+                    gg += hp.weight_decay * wv[k];
+                av[k] = hp.beta1 * av[k] + (1.f - hp.beta1) * gg;
+                bv[k] = hp.beta2 * bv[k] + (1.f - hp.beta2) * gg * gg;
+                const float denom = sqrtf(bv[k]) * l.inv_sqrt_bc2 + hp.eps;
+                wv[k] -= (hp.lr * l.inv_bc1) * (av[k] / denom);
+                w[4 * q + k] = wv[k];
+            }
+            wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
+            ap[q] = make_float4(av[0], av[1], av[2], av[3]);
+            bp[q] = make_float4(bv[0], bv[1], bv[2], bv[3]);
+        }
+    }
+};
+
+// Lion (lion.cuh): x[k]·coef is the gradient, the fp32 master and exp_avg are updated in place; one moment instead of Adam's two, so
+// 16 bytes of state per owned element instead of 24. No step-dependent parameter.
+template <>
+struct Update<LionRule> : LionRule {
+    struct Local {};
+    __device__ __forceinline__ static Local setup(const Params&) { return {}; }
+    __device__ __forceinline__ static void at_step(Params&, uint32_t) {}
+    __device__ __forceinline__ const float* source(const float* shard) const { return shard; }
+    __device__ __forceinline__ float coef(const float* c) const { return *c; }
+    template <int N>
+    __device__ __forceinline__ void update(Local&, const Params& hp, size_t j, const float* x, float coef, float* w) const {
+        float4* wp = reinterpret_cast<float4*>(master + j * N);
+        float4* mp = reinterpret_cast<float4*>(exp_avg + j * N);
+#pragma unroll
+        for (int q = 0; q < N / 4; ++q) {
+            const float4 ww = wp[q], mm = mp[q];
+            float wv[4] = {ww.x, ww.y, ww.z, ww.w}, mv[4] = {mm.x, mm.y, mm.z, mm.w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                lion_apply(wv[k], mv[k], lion_grad(x[4 * q + k], coef), hp);
+                w[4 * q + k] = wv[k];
+            }
+            wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
+            mp[q] = make_float4(mv[0], mv[1], mv[2], mv[3]);
+        }
+    }
+};
+
+// segs = [nsegs][lo, hi, param] sorted by lo, disjoint, with gaps where the padding tensor lies. The last segment with lo ≤ e
+// (−1: none), by bisection; the LAMB and LARS walks find it once per vector and advance it element by element, since a 16-byte
+// vector may hold elements of several parameters.
+__device__ __forceinline__ int lamb_segment_at(const int32_t* segs, int nsegs, int64_t e) {
+    int lo = 0, hi = nsegs;  // first segment with lo > e
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (segs[3 * mid] <= e) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo - 1;
 }
 
+// LAMB's apply (phase B only, see lamb_ratio_kernel): w ← w − lr·r·u over the fp32 master, u recomputed from the stage-1 moments
+// (lamb_direction, the same code that fed Σu²), r = ratio of the element's parameter (1 in the gaps of the segment table). The bias
+// corrections at_step builds are the ones the moments kernel built from the same t. There is no gradient coefficient: with a vote,
+// the kernel's coef is only the {coef, found_inf} pair the vote is read from.
+template <>
+struct Update<LambRule> : LambRule {
+    struct Local {};
+    __device__ __forceinline__ static Local setup(const Params&) { return {}; }
+    __device__ __forceinline__ static void at_step(Params& hp, uint32_t t) {
+        hp.bias_correction1 = bias_correction(hp.beta1, t);
+        hp.bias_correction2 = bias_correction(hp.beta2, t);
+    }
+    __device__ __forceinline__ const float* source(const float*) const { return master; }
+    __device__ __forceinline__ float coef(const float*) const { return 1.f; }
+    template <int N>
+    __device__ __forceinline__ void update(Local&, const Params& hp, size_t j, const float* w0, float, float* w) const {
+        const float4* ap = reinterpret_cast<const float4*>(exp_avg + j * N);
+        const float4* bp = reinterpret_cast<const float4*>(exp_avg_sq + j * N);
+        int s = lamb_segment_at(segs, nsegs, static_cast<int64_t>(j * N));
+#pragma unroll
+        for (int q = 0; q < N / 4; ++q) {
+            const float4 aa = ap[q], bb = bp[q];
+            const float av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int64_t e = static_cast<int64_t>(j * N + 4 * q + k);
+                while (s + 1 < nsegs && segs[3 * (s + 1)] <= e) ++s;
+                const float r = (s >= 0 && e < segs[3 * s + 1]) ? ratio[segs[3 * s + 2]] : 1.f;
+                w[4 * q + k] = lamb_apply(w0[4 * q + k], lamb_direction(w0[4 * q + k], av[k], bv[k], hp), r, hp);
+            }
+        }
+        float4* wp = reinterpret_cast<float4*>(master + j * N);
+#pragma unroll
+        for (int q = 0; q < N / 4; ++q) wp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+    }
+};
+
+// LARS's momentum and apply (phase B only, the program of LAMB with a different pair: multi_tensor_lars_stage1 leaves fp64
+// {Σw², Σg̃²} per block, lamb_ratio_kernel exchanges them per parameter into sums) from the gradient shard·coef (lars_grad, the code
+// that fed Σg̃²; a null coef is 1). The trust of an element's parameter comes from the exchanged global sums and is taken again only
+// when the walk enters another parameter (1 in the gaps of the segment table). No step-dependent parameter.
+template <>
+struct Update<LarsRule> : LarsRule {
+    struct Local {
+        float lt = 0.f;
+        int cur = -2;  // parameter whose step size lt holds (−1: a gap)
+    };
+    __device__ __forceinline__ static Local setup(const Params&) { return {}; }
+    __device__ __forceinline__ static void at_step(Params&, uint32_t) {}
+    __device__ __forceinline__ const float* source(const float* shard) const { return shard; }
+    __device__ __forceinline__ float coef(const float* c) const { return c != nullptr ? *c : 1.f; }
+    template <int N>
+    __device__ __forceinline__ void update(Local& l, const Params& hp, size_t j, const float* g, float c, float* w) const {
+        float4* mp = reinterpret_cast<float4*>(master + j * N);
+        float4* vp = reinterpret_cast<float4*>(momentum + j * N);
+        int s = lamb_segment_at(segs, nsegs, static_cast<int64_t>(j * N));
+#pragma unroll
+        for (int q = 0; q < N / 4; ++q) {
+            const float4 ww = mp[q], vv = vp[q];
+            float wv[4] = {ww.x, ww.y, ww.z, ww.w}, v[4] = {vv.x, vv.y, vv.z, vv.w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int64_t e = static_cast<int64_t>(j * N + 4 * q + k);
+                while (s + 1 < nsegs && segs[3 * (s + 1)] <= e) ++s;
+                const int t = (s >= 0 && e < segs[3 * s + 1]) ? segs[3 * s + 2] : -1;
+                if (t != l.cur) {
+                    l.cur = t;
+                    l.lt = lars_step_size(t >= 0 ? lars_trust(sums[2 * t], sums[2 * t + 1], hp) : 1.f, hp);
+                }
+                lars_apply(wv[k], v[k], lars_grad(g[4 * q + k], c), l.lt, hp);
+                w[4 * q + k] = wv[k];
+            }
+            mp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
+            vp[q] = make_float4(v[0], v[1], v[2], v[3]);
+        }
+    }
+};
+
 // ---------------------------------------------------------------------------------------------------------
-// Gradient reduce-scatter  →  SGD(momentum) on the owned 1/P slice  →  all-gather of the updated WEIGHTS,
-// in one kernel. Each rank keeps fp32 master weights and momentum only for its own slice (optimizer state is
-// sharded P ways), the gradient bucket is zeroed for the next iteration on the way out, and the optimizer step
-// overlaps the rest of backward because it runs inside the bucket's communication kernel.
+// Gradient reduce-scatter  →  the rule (SGD, Adam, Lion) on the owned 1/P slice  →  all-gather of the updated WEIGHTS, in one
+// kernel. Each rank keeps the fp32 master weights and the optimizer state only for its own slice (optimizer state is sharded P ways),
+// the gradient bucket is zeroed for the next iteration on the way out, and the optimizer step overlaps the rest of backward because it
+// runs inside the bucket's communication kernel.
 // ---------------------------------------------------------------------------------------------------------
-template <typename T, int P, bool USE_MC>
+template <typename T, int P, bool USE_MC, class R, class... State>
 __global__ void __launch_bounds__(512)
-    allreduce_sgd_kernel(PeerCtx ctx, PeerBuf grads, PeerBuf weights, size_t g_off, size_t w_off, size_t total_vecs,
-                         float* master, float* momentum_buf, SgdParams hp, float scale, int zero_grads) {
+    allreduce_update_kernel(PeerCtx ctx, PeerBuf grads, PeerBuf weights, size_t g_off, size_t w_off, size_t total_vecs, State... state,
+                            typename R::Params hp, float scale, int zero_grads) {
+    const Update<R> rule{{state...}};
     const uint32_t e0 = load_epoch(ctx);
     bool ok = peer_barrier(ctx, e0 + 1);
     constexpr int N = Vec16<T>::N;
     const Slicing sl(total_vecs, P);
     if (ok) {
+        auto local = rule.setup(hp);
         reduce_owned_slice<T, P, USE_MC, kOptimizerUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t v, size_t j, float* g) {
             float w[N];
-            sgd_update<N>(master, momentum_buf, j, g, scale, hp, w);
+            rule.template update<N>(local, hp, j, g, scale, w);
             publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
         });
         ok = peer_barrier(ctx, e0 + 2);
@@ -332,90 +483,15 @@ __global__ void __launch_bounds__(512)
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// The same reduce-scatter → optimizer → all-gather kernel with Adam / AdamW on the owned shard (fp32 master weights and
-// both moments sharded P ways). Update rule identical to flat_adam_kernel (multi_tensor.cu) / torch.optim.Adam[W].
-// ---------------------------------------------------------------------------------------------------------
-template <typename T, int P, bool USE_MC>
-__global__ void __launch_bounds__(512)
-    allreduce_adam_kernel(PeerCtx ctx, PeerBuf grads, PeerBuf weights, size_t g_off, size_t w_off, size_t total_vecs, float* master,
-                          float* exp_avg, float* exp_avg_sq, AdamParams hp, float scale, int zero_grads) {
-    const uint32_t e0 = load_epoch(ctx);
-    bool ok = peer_barrier(ctx, e0 + 1);
-    constexpr int N = Vec16<T>::N;
-    const Slicing sl(total_vecs, P);
-    if (ok) {
-        const float inv_bc1 = 1.f / hp.bias_correction1, inv_sqrt_bc2 = rsqrtf(hp.bias_correction2);
-        reduce_owned_slice<T, P, USE_MC, kOptimizerUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t v, size_t j, float* g) {
-            float w[N];
-            adam_update<N>(master, exp_avg, exp_avg_sq, j, g, scale, hp, inv_bc1, inv_sqrt_bc2, w);
-            publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
-        });
-        ok = peer_barrier(ctx, e0 + 2);
-    }
-    if (ok && zero_grads) {
-        char* mine = grads.ptr[ctx.rank] + g_off;
-        for_each_striped<P>(sl, [&](size_t v) { st_stream16(mine + v * 16, make_uint4(0, 0, 0, 0)); });
-    }
-    store_epoch(ctx, e0 + 2);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Lion on one 16-byte vector of the owned shard (lion.cuh): x[k]·coef is the gradient, the fp32 master and exp_avg are updated in
-// place and w receives the new weights, which the caller publishes.
-// ---------------------------------------------------------------------------------------------------------
-template <int N>
-__device__ __forceinline__ void lion_update(float* master, float* exp_avg, size_t j, const float* x, float coef, const LionParams& hp, float* w) {
-    float4* wp = reinterpret_cast<float4*>(master + j * N);
-    float4* mp = reinterpret_cast<float4*>(exp_avg + j * N);
-#pragma unroll
-    for (int q = 0; q < N / 4; ++q) {
-        const float4 ww = wp[q], mm = mp[q];
-        float wv[4] = {ww.x, ww.y, ww.z, ww.w}, mv[4] = {mm.x, mm.y, mm.z, mm.w};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            lion_apply(wv[k], mv[k], lion_grad(x[4 * q + k], coef), hp);
-            w[4 * q + k] = wv[k];
-        }
-        wp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
-        mp[q] = make_float4(mv[0], mv[1], mv[2], mv[3]);
-    }
-}
-
-// The reduce-scatter → optimizer → all-gather kernel of allreduce_adam_kernel with Lion on the owned shard (fp32 master weights and
-// exp_avg sharded P ways): one moment instead of two, so 16 bytes of state per owned element instead of 24.
-template <typename T, int P, bool USE_MC>
-__global__ void __launch_bounds__(512)
-    allreduce_lion_kernel(PeerCtx ctx, PeerBuf grads, PeerBuf weights, size_t g_off, size_t w_off, size_t total_vecs, float* master, float* exp_avg,
-                          LionParams hp, float scale, int zero_grads) {
-    const uint32_t e0 = load_epoch(ctx);
-    bool ok = peer_barrier(ctx, e0 + 1);
-    constexpr int N = Vec16<T>::N;
-    const Slicing sl(total_vecs, P);
-    if (ok) {
-        reduce_owned_slice<T, P, USE_MC, kOptimizerUnroll<P, USE_MC>>(ctx, grads, g_off, sl, [&](size_t v, size_t j, float* g) {
-            float w[N];
-            lion_update<N>(master, exp_avg, j, g, scale, hp, w);
-            publish16<P, USE_MC>(ctx, weights, w_off, v, Vec16<T>::pack(w));
-        });
-        ok = peer_barrier(ctx, e0 + 2);
-    }
-    if (ok && zero_grads) {
-        char* mine = grads.ptr[ctx.rank] + g_off;
-        for_each_striped<P>(sl, [&](size_t v) { st_stream16(mine + v * 16, make_uint4(0, 0, 0, 0)); });
-    }
-    store_epoch(ctx, e0 + 2);
-}
-
-// ---------------------------------------------------------------------------------------------------------
 // Global-norm gradient clipping for the in-bucket optimizers. No shard may be updated before the norm over every bucket of every
 // rank is known, so the single in-bucket kernel above becomes two phases around a norm exchange:
 //   A  shard_grad_kernel, per bucket, inside backward on the comm stream: the owned-slice reduction (same order and the same
-//      multimem / peer ld choice as allreduce_{sgd,adam}_kernel) scaled by `scale` → the fp32 gradient of the owned slice in
+//      multimem / peer ld choice as allreduce_update_kernel) scaled by `scale` → the fp32 gradient of the owned slice in
 //      `shard`; one fp64 Σx² per CTA in partials[block] (no atomics: reproducible, nothing to reset between steps); the bucket is
 //      cleared after the closing barrier.
 //   N  grad_norm_kernel, once per step: the rank's Σ over all partials (+ the parameters outside the buckets) → slot [rank] of
 //      every peer's norm box → barrier → Σ over slots 0 .. P-1 in rank order, so every rank computes the same bits → total, coef.
-//   B  shard_{sgd,adam}_kernel, per bucket: the update of the shard scaled by coef (read from device memory: the host never sees
+//   B  shard_update_kernel, per bucket: the update of the shard scaled by coef (read from device memory: the host never sees
 //      the norm) → all-gather of the weights → closing barrier, so no rank's trainer reads weights a peer is still writing.
 // With ACCUM (gradient accumulation over micro-batches) phase A adds into the shard instead of overwriting it:
 // s ← fl32(s_old + fl32(red·scale)), the product and the sum rounded separately (no FMA), and Σx² is taken over the new s. Every
@@ -623,64 +699,29 @@ __device__ __forceinline__ void update_owned_shard(const PeerCtx& ctx, const Pee
         });
 }
 
+// Phase B of every rule: the update of the owned shard from rule.source(shard) with the coefficient rule.coef(coef), the all-gather of
+// the weights, the closing barrier.
 //
-// DEV_STEP (loss scaling): `coef` addresses {coef, found_inf} of loss_scale_norm_kernel and *step is the effective step count t that
+// VOTE (loss scaling): `coef` addresses {coef, found_inf} of loss_scale_norm_kernel and *step is the effective step count t that
 // includes this step. The vote has the same bits on every rank, so the branch on it is uniform across ranks and CTAs: a skipped step
-// touches no state, publishes nothing and only takes the closing barrier; a taken one rebuilds the step-dependent fields of hp from
-// t. Without DEV_STEP `step` is not read and hp is the host's.
-template <typename T, int P, bool USE_MC, bool DEV_STEP>
-__global__ void __launch_bounds__(512) shard_sgd_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
-                                                        const float* coef, float* master, float* momentum_buf, SgdParams hp, const uint32_t* step) {
+// touches no state, publishes nothing and only takes the closing barrier; a taken one rebuilds the step-dependent fields of the rule
+// from t. Without VOTE `step` is not read and the rule's parameters are the host's.
+template <typename T, int P, bool USE_MC, bool VOTE, class R, class... State>
+__global__ void __launch_bounds__(512) shard_update_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
+                                                           const float* coef, State... state, typename R::Params hp, const uint32_t* step) {
+    const Update<R> rule{{state...}};
     const uint32_t e0 = load_epoch(ctx);
-    const float c = *coef;
+    const float c = rule.coef(coef);
     bool skip = false;
-    if constexpr (DEV_STEP) {
+    if constexpr (VOTE) {
         skip = coef[1] != 0.f;
-        hp.first_step = *step == 1u ? 1 : 0;
-    }
-    if (!skip)
-        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard,
-                                         [&](size_t j, const float* g, float* w) { sgd_update<Vec16<T>::N>(master, momentum_buf, j, g, c, hp, w); });
-    peer_barrier(ctx, e0 + 1);
-    store_epoch(ctx, e0 + 1);
-}
-
-template <typename T, int P, bool USE_MC, bool DEV_STEP>
-__global__ void __launch_bounds__(512) shard_adam_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
-                                                         const float* coef, float* master, float* exp_avg, float* exp_avg_sq, AdamParams hp,
-                                                         const uint32_t* step) {
-    const uint32_t e0 = load_epoch(ctx);
-    const float c = *coef;
-    bool skip = false;
-    if constexpr (DEV_STEP) {
-        skip = coef[1] != 0.f;
-        const uint32_t t = *step;
-        hp.bias_correction1 = bias_correction(hp.beta1, t);
-        hp.bias_correction2 = bias_correction(hp.beta2, t);
+        rule.at_step(hp, *step);
     }
     if (!skip) {
-        const float inv_bc1 = 1.f / hp.bias_correction1, inv_sqrt_bc2 = rsqrtf(hp.bias_correction2);
-        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard, [&](size_t j, const float* g, float* w) {
-            adam_update<Vec16<T>::N>(master, exp_avg, exp_avg_sq, j, g, c, hp, inv_bc1, inv_sqrt_bc2, w);
-        });
+        auto local = rule.setup(hp);
+        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), rule.source(shard),
+                                         [&](size_t j, const float* g, float* w) { rule.template update<Vec16<T>::N>(local, hp, j, g, c, w); });
     }
-    peer_barrier(ctx, e0 + 1);
-    store_epoch(ctx, e0 + 1);
-}
-
-// Phase B of the in-bucket Lion: the update of the owned shard from the gradient shard·*coef. Lion has no step-dependent parameter,
-// so loss scaling needs only the vote: with VOTE coef addresses {coef, found_inf} and a skipped step touches no state, publishes
-// nothing and only takes the closing barrier.
-template <typename T, int P, bool USE_MC, bool VOTE>
-__global__ void __launch_bounds__(512) shard_lion_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
-                                                         const float* coef, float* master, float* exp_avg, LionParams hp) {
-    const uint32_t e0 = load_epoch(ctx);
-    const float c = *coef;
-    bool skip = false;
-    if constexpr (VOTE) skip = coef[1] != 0.f;
-    if (!skip)
-        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard,
-                                         [&](size_t j, const float* g, float* w) { lion_update<Vec16<T>::N>(master, exp_avg, j, g, c, hp, w); });
     peer_barrier(ctx, e0 + 1);
     store_epoch(ctx, e0 + 1);
 }
@@ -688,7 +729,7 @@ __global__ void __launch_bounds__(512) shard_lion_kernel(PeerCtx ctx, PeerBuf we
 // ---------------------------------------------------------------------------------------------------------
 // In-bucket LAMB. Its trust ratio is a norm over a whole parameter, and the owned slices cut parameters anywhere, so after phase A
 // (shard_grad_kernel, unchanged) step() runs: the moments of each shard (multi_tensor_lamb_stage1 over the shard's segments, one
-// parameter ∩ owned slice each, leaving fp64 {Σw², Σu²} per block) → lamb_ratio_kernel, once per step → shard_lamb_kernel per bucket.
+// parameter ∩ owned slice each, leaving fp64 {Σw², Σu²} per block) → lamb_ratio_kernel, once per step → shard_update_kernel per bucket.
 //
 // lamb_ratio_kernel, one CTA: parameter t's local pair is the sum of its segment's block pairs in block order; the pairs go to slot
 // [rank][t] of every peer's box, double-buffered by the op's call counter like grad_norm_kernel (a rank writes a half again two calls
@@ -728,105 +769,6 @@ __global__ void __launch_bounds__(kRatioThreads) lamb_ratio_kernel(PeerCtx ctx, 
     store_epoch(ctx, e0 + 1);
 }
 
-// segs = [nsegs][lo, hi, param] sorted by lo, disjoint, with gaps where the padding tensor lies. The last segment with lo ≤ e
-// (−1: none), by bisection; the walk below finds it once per vector and advances it element by element, since a 16-byte vector may
-// hold elements of several parameters.
-__device__ __forceinline__ int lamb_segment_at(const int32_t* segs, int nsegs, int64_t e) {
-    int lo = 0, hi = nsegs;  // first segment with lo > e
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (segs[3 * mid] <= e) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo - 1;
-}
-
-// Apply and publish: w ← w − lr·r·u on the owned slice with u recomputed from the stage-1 moments (lamb_direction, the same code
-// that fed Σu²), all-gather of the weights, closing barrier — the walk of shard_adam_kernel over the fp32 master. DEV_STEP as for
-// shard_sgd_kernel, with vote = {coef, found_inf}: the bias corrections are the ones the moments kernel built from the same t.
-template <typename T, int P, bool USE_MC, bool DEV_STEP>
-__global__ void __launch_bounds__(512) shard_lamb_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, float* master, const float* exp_avg,
-                                                         const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, LambParams hp,
-                                                         const float* vote, const uint32_t* step) {
-    const uint32_t e0 = load_epoch(ctx);
-    constexpr int N = Vec16<T>::N;
-    bool skip = false;
-    if constexpr (DEV_STEP) {
-        skip = vote[1] != 0.f;
-        const uint32_t t = *step;
-        hp.bias_correction1 = bias_correction(hp.beta1, t);
-        hp.bias_correction2 = bias_correction(hp.beta2, t);
-    }
-    if (!skip) update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), master, [&](size_t j, const float* w0, float* w) {
-        const float4* ap = reinterpret_cast<const float4*>(exp_avg + j * N);
-        const float4* bp = reinterpret_cast<const float4*>(exp_avg_sq + j * N);
-        int s = lamb_segment_at(segs, nsegs, static_cast<int64_t>(j * N));
-#pragma unroll
-        for (int q = 0; q < N / 4; ++q) {
-            const float4 aa = ap[q], bb = bp[q];
-            const float av[4] = {aa.x, aa.y, aa.z, aa.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const int64_t e = static_cast<int64_t>(j * N + 4 * q + k);
-                while (s + 1 < nsegs && segs[3 * (s + 1)] <= e) ++s;
-                const float r = (s >= 0 && e < segs[3 * s + 1]) ? ratio[segs[3 * s + 2]] : 1.f;
-                w[4 * q + k] = lamb_apply(w0[4 * q + k], lamb_direction(w0[4 * q + k], av[k], bv[k], hp), r, hp);
-            }
-        }
-        float4* wp = reinterpret_cast<float4*>(master + j * N);
-#pragma unroll
-        for (int q = 0; q < N / 4; ++q) wp[q] = make_float4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-    });
-    peer_barrier(ctx, e0 + 1);
-    store_epoch(ctx, e0 + 1);
-}
-
-// In-bucket LARS, the program of LAMB with a different pair: multi_tensor_lars_stage1 over the shard's segments leaves fp64
-// {Σw², Σg̃²} per block, lamb_ratio_kernel exchanges them per parameter into sums (its ratio output goes unused), and this kernel
-// applies momentum and update to the owned slice from the gradient shard·coef (lars_grad, the code that fed Σg̃²), then all-gathers
-// the weights and takes the closing barrier. The trust of an element's parameter comes from the exchanged global sums and is taken
-// again only when the walk enters another parameter (1 in the gaps of the segment table). VOTE: coef addresses {coef, found_inf};
-// a skipped step goes straight to the closing barrier.
-template <typename T, int P, bool USE_MC, bool VOTE>
-__global__ void __launch_bounds__(512) shard_lars_kernel(PeerCtx ctx, PeerBuf weights, size_t w_off, size_t total_vecs, const float* shard,
-                                                         const float* coef, float* master, float* momentum, const int32_t* segs, int nsegs,
-                                                         const double* sums, LarsParams hp) {
-    const uint32_t e0 = load_epoch(ctx);
-    constexpr int N = Vec16<T>::N;
-    const float c = coef != nullptr ? *coef : 1.f;
-    bool skip = false;
-    if constexpr (VOTE) skip = coef[1] != 0.f;
-    if (!skip) {
-        int cur = -2;    // parameter whose step size lt holds (−1: a gap)
-        float lt = 0.f;
-        update_owned_shard<T, P, USE_MC>(ctx, weights, w_off, Slicing(total_vecs, P), shard, [&](size_t j, const float* g, float* w) {
-            float4* mp = reinterpret_cast<float4*>(master + j * N);
-            float4* vp = reinterpret_cast<float4*>(momentum + j * N);
-            int s = lamb_segment_at(segs, nsegs, static_cast<int64_t>(j * N));
-#pragma unroll
-            for (int q = 0; q < N / 4; ++q) {
-                const float4 ww = mp[q], vv = vp[q];
-                float wv[4] = {ww.x, ww.y, ww.z, ww.w}, v[4] = {vv.x, vv.y, vv.z, vv.w};
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const int64_t e = static_cast<int64_t>(j * N + 4 * q + k);
-                    while (s + 1 < nsegs && segs[3 * (s + 1)] <= e) ++s;
-                    const int t = (s >= 0 && e < segs[3 * s + 1]) ? segs[3 * s + 2] : -1;
-                    if (t != cur) {
-                        cur = t;
-                        lt = lars_step_size(t >= 0 ? lars_trust(sums[2 * t], sums[2 * t + 1], hp) : 1.f, hp);
-                    }
-                    lars_apply(wv[k], v[k], lars_grad(g[4 * q + k], c), lt, hp);
-                    w[4 * q + k] = wv[k];
-                }
-                mp[q] = make_float4(wv[0], wv[1], wv[2], wv[3]);
-                vp[q] = make_float4(v[0], v[1], v[2], v[3]);
-            }
-        });
-    }
-    peer_barrier(ctx, e0 + 1);
-    store_epoch(ctx, e0 + 1);
-}
 
 // Publication of an fp32 shard as the bucket's weights: the walk of the update kernels with a copy in place of the update, so
 // Vec16<T>::pack(src) lands in every rank's copy of the owned slice. The weight EMA swaps its shard in with it and the master back
@@ -1049,6 +991,13 @@ size_t peer_vecs(const char* what, size_t bytes, size_t off_a, size_t off_b, int
     if (nblocks < 1 || nblocks > kMaxCommBlocks) throw std::runtime_error("bagua: peer kernel grid must be 1.." + std::to_string(kMaxCommBlocks));
     return bytes / 16;
 }
+
+// The checks of a rule's parameters, made by both of its launchers.
+template <class Params>
+void check_params(const char*, const Params&) {}
+void check_params(const char* what, const AdamParams& hp) {
+    if (hp.amsgrad) throw std::runtime_error(std::string("bagua: ") + what + " does not implement amsgrad");
+}
 }  // namespace
 
 void launch_allreduce(const PeerCtx& ctx, const PeerBuf& src, const PeerBuf& dst, size_t src_off, size_t dst_off,
@@ -1083,21 +1032,6 @@ void launch_allreduce_oneshot(const PeerCtx& ctx, const PeerBuf& staging, size_t
     check_launch("allreduce_oneshot");
 }
 
-void launch_allreduce_sgd(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off,
-                          size_t bytes, int dtype, float* master, float* momentum, const SgdParams& hp, float scale,
-                          bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream) {
-    const size_t vecs = peer_vecs("allreduce_sgd", bytes, g_off, w_off, nblocks);
-    if (vecs == 0) return;
-    dispatch_float(dtype, kFamily, [&](auto tag) {
-        dispatch_world(ctx.world, [&](auto pw) {
-            dispatch_mc(use_multimem, [&](auto mc) {
-                allreduce_sgd_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
-                    ctx, grads, weights, g_off, w_off, vecs, master, momentum, hp, scale, zero_grads ? 1 : 0);
-            });
-        });
-    });
-    check_launch("allreduce_sgd");
-}
 
 void launch_reduce_scatter(const PeerCtx& ctx, const PeerBuf& buf, size_t off, size_t bytes, int dtype, float scale, bool use_multimem, int nblocks,
                            int nthreads, cudaStream_t stream) {
@@ -1128,56 +1062,6 @@ void launch_all_gather(const PeerCtx& ctx, const PeerBuf& buf, size_t off, size_
     check_launch("all_gather");
 }
 
-void launch_allreduce_adam(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
-                           float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, float scale, bool zero_grads, bool use_multimem,
-                           int nblocks, int nthreads, cudaStream_t stream) {
-    const size_t vecs = peer_vecs("allreduce_adam", bytes, g_off, w_off, nblocks);
-    if (hp.amsgrad) throw std::runtime_error("bagua: allreduce_adam does not implement amsgrad");
-    if (vecs == 0) return;
-    dispatch_float(dtype, kFamily, [&](auto tag) {
-        dispatch_world(ctx.world, [&](auto pw) {
-            dispatch_mc(use_multimem, [&](auto mc) {
-                allreduce_adam_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
-                    ctx, grads, weights, g_off, w_off, vecs, master, exp_avg, exp_avg_sq, hp, scale, zero_grads ? 1 : 0);
-            });
-        });
-    });
-    check_launch("allreduce_adam");
-}
-
-void launch_allreduce_lion(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
-                           float* master, float* exp_avg, const LionParams& hp, float scale, bool zero_grads, bool use_multimem, int nblocks, int nthreads,
-                           cudaStream_t stream) {
-    const size_t vecs = peer_vecs("allreduce_lion", bytes, g_off, w_off, nblocks);
-    if (vecs == 0) return;
-    dispatch_float(dtype, kFamily, [&](auto tag) {
-        dispatch_world(ctx.world, [&](auto pw) {
-            dispatch_mc(use_multimem, [&](auto mc) {
-                allreduce_lion_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value><<<nblocks, nthreads, 0, stream>>>(
-                    ctx, grads, weights, g_off, w_off, vecs, master, exp_avg, hp, scale, zero_grads ? 1 : 0);
-            });
-        });
-    });
-    check_launch("allreduce_lion");
-}
-
-void launch_shard_lion(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                       float* master, float* exp_avg, const LionParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream, bool vote) {
-    const size_t vecs = peer_vecs("shard_lion", bytes, w_off, 0, nblocks);
-    if (coef == nullptr) throw std::runtime_error("bagua: shard_lion needs a gradient coefficient ({coef, found_inf} with a vote)");
-    if (vecs == 0) return;
-    dispatch_float(dtype, kFamily, [&](auto tag) {
-        dispatch_world(ctx.world, [&](auto pw) {
-            dispatch_mc(use_multimem, [&](auto mc) {
-                dispatch_flag(vote, [&](auto vt) {
-                    shard_lion_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(vt)::value><<<nblocks, nthreads, 0, stream>>>(
-                        ctx, weights, w_off, vecs, shard, coef, master, exp_avg, hp);
-                });
-            });
-        });
-    });
-    check_launch("shard_lion");
-}
 
 void launch_shard_grad(const PeerCtx& ctx, const PeerBuf& grads, size_t g_off, size_t bytes, int dtype, float* shard, double* partials, float scale,
                        bool zero_grads, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream, bool accumulate) {
@@ -1226,42 +1110,6 @@ void launch_loss_scale_norm(const PeerCtx& ctx, const PeerBuf& box, size_t box_o
     check_launch("loss_scale_norm");
 }
 
-void launch_shard_sgd(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                      float* master, float* momentum, const SgdParams& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream,
-                      const uint32_t* step) {
-    const size_t vecs = peer_vecs("shard_sgd", bytes, w_off, 0, nblocks);
-    if (vecs == 0) return;
-    dispatch_float(dtype, kFamily, [&](auto tag) {
-        dispatch_world(ctx.world, [&](auto pw) {
-            dispatch_mc(use_multimem, [&](auto mc) {
-                dispatch_flag(step != nullptr, [&](auto dev) {
-                    shard_sgd_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(dev)::value><<<nblocks, nthreads, 0, stream>>>(
-                        ctx, weights, w_off, vecs, shard, coef, master, momentum, hp, step);
-                });
-            });
-        });
-    });
-    check_launch("shard_sgd");
-}
-
-void launch_shard_adam(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                       float* master, float* exp_avg, float* exp_avg_sq, const AdamParams& hp, bool use_multimem, int nblocks, int nthreads,
-                       cudaStream_t stream, const uint32_t* step) {
-    const size_t vecs = peer_vecs("shard_adam", bytes, w_off, 0, nblocks);
-    if (hp.amsgrad) throw std::runtime_error("bagua: shard_adam does not implement amsgrad");
-    if (vecs == 0) return;
-    dispatch_float(dtype, kFamily, [&](auto tag) {
-        dispatch_world(ctx.world, [&](auto pw) {
-            dispatch_mc(use_multimem, [&](auto mc) {
-                dispatch_flag(step != nullptr, [&](auto dev) {
-                    shard_adam_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(dev)::value><<<nblocks, nthreads, 0, stream>>>(
-                        ctx, weights, w_off, vecs, shard, coef, master, exp_avg, exp_avg_sq, hp, step);
-                });
-            });
-        });
-    });
-    check_launch("shard_adam");
-}
 
 void launch_lamb_ratio(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, const uint64_t* seg_ptr, const int32_t* seg_nblk, int nparams,
                        uint32_t parity, float* ratio, double* sums, cudaStream_t stream) {
@@ -1271,43 +1119,75 @@ void launch_lamb_ratio(const PeerCtx& ctx, const PeerBuf& box, size_t box_off, c
     check_launch("lamb_ratio");
 }
 
-void launch_shard_lamb(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, float* master, const float* exp_avg,
-                       const float* exp_avg_sq, const int32_t* segs, int nsegs, const float* ratio, const LambParams& hp, bool use_multimem,
-                       int nblocks, int nthreads, cudaStream_t stream, const float* vote, const uint32_t* step) {
-    const size_t vecs = peer_vecs("shard_lamb", bytes, w_off, 0, nblocks);
-    if ((vote == nullptr) != (step == nullptr)) throw std::runtime_error("bagua: shard_lamb takes the vote and the step counter together");
+template <class R>
+void launch_fused_update(const PeerCtx& ctx, const PeerBuf& grads, const PeerBuf& weights, size_t g_off, size_t w_off, size_t bytes, int dtype,
+                         const R& rule, const typename R::Params& hp, float scale, bool zero_grads, bool use_multimem, int nblocks, int nthreads,
+                         cudaStream_t stream) {
+    const size_t vecs = peer_vecs(R::kFused, bytes, g_off, w_off, nblocks);
+    check_params(R::kFused, hp);
     if (vecs == 0) return;
     dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
             dispatch_mc(use_multimem, [&](auto mc) {
-                dispatch_flag(step != nullptr, [&](auto dev) {
-                    shard_lamb_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(dev)::value><<<nblocks, nthreads, 0, stream>>>(
-                        ctx, weights, w_off, vecs, master, exp_avg, exp_avg_sq, segs, nsegs, ratio, hp, vote, step);
-                });
+                std::apply(
+                    [&](auto... state) {
+                        allreduce_update_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, R, decltype(state)...><<<nblocks, nthreads, 0, stream>>>(
+                            ctx, grads, weights, g_off, w_off, vecs, state..., hp, scale, zero_grads ? 1 : 0);
+                    },
+                    rule.fields());
             });
         });
     });
-    check_launch("shard_lamb");
+    check_launch(R::kFused);
 }
+#define BAGUA_FUSED_UPDATE(R)                                                                                                                     \
+    template void launch_fused_update(const PeerCtx&, const PeerBuf&, const PeerBuf&, size_t, size_t, size_t, int, const R&, const R::Params&, float, bool, bool, int, \
+                                      int, cudaStream_t);
+BAGUA_FUSED_UPDATE(SgdRule)
+BAGUA_FUSED_UPDATE(AdamRule)
+BAGUA_FUSED_UPDATE(LionRule)
+#undef BAGUA_FUSED_UPDATE
 
-void launch_shard_lars(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
-                       float* master, float* momentum, const int32_t* segs, int nsegs, const double* sums, const LarsParams& hp, bool use_multimem,
-                       int nblocks, int nthreads, cudaStream_t stream, bool vote) {
-    const size_t vecs = peer_vecs("shard_lars", bytes, w_off, 0, nblocks);
-    if (vote && coef == nullptr) throw std::runtime_error("bagua: shard_lars with a vote needs {coef, found_inf}");
+template <class R>
+void launch_shard_update(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* shard, const float* coef,
+                         const R& rule, const typename R::Params& hp, bool use_multimem, int nblocks, int nthreads, cudaStream_t stream,
+                         const uint32_t* step) {
+    const size_t vecs = peer_vecs(R::kShard, bytes, w_off, 0, nblocks);
+    check_params(R::kShard, hp);
+    if (step != nullptr && coef == nullptr) throw std::runtime_error(std::string("bagua: ") + R::kShard + " with a vote needs {coef, found_inf}");
+    if constexpr (std::is_same_v<R, LionRule>) {
+        if (coef == nullptr) throw std::runtime_error("bagua: shard_lion needs a gradient coefficient ({coef, found_inf} with a vote)");
+    }
+    if constexpr (std::is_same_v<R, LambRule>) {  // LAMB reads no coefficient: its coef is the vote
+        if (coef != nullptr && step == nullptr) throw std::runtime_error("bagua: shard_lamb takes the vote and the step counter together");
+    }
     if (vecs == 0) return;
     dispatch_float(dtype, kFamily, [&](auto tag) {
         dispatch_world(ctx.world, [&](auto pw) {
             dispatch_mc(use_multimem, [&](auto mc) {
-                dispatch_flag(vote, [&](auto vt) {
-                    shard_lars_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(vt)::value><<<nblocks, nthreads, 0, stream>>>(
-                        ctx, weights, w_off, vecs, shard, coef, master, momentum, segs, nsegs, sums, hp);
+                dispatch_flag(step != nullptr, [&](auto vote) {
+                    std::apply(
+                        [&](auto... state) {
+                            shard_update_kernel<decltype(tag), decltype(pw)::value, decltype(mc)::value, decltype(vote)::value, R, decltype(state)...>
+                                <<<nblocks, nthreads, 0, stream>>>(ctx, weights, w_off, vecs, shard, coef, state..., hp, step);
+                        },
+                        rule.fields());
                 });
             });
         });
     });
-    check_launch("shard_lars");
+    check_launch(R::kShard);
 }
+#define BAGUA_SHARD_UPDATE(R)                                                                                                                    \
+    template void launch_shard_update(const PeerCtx&, const PeerBuf&, size_t, size_t, int, const float*, const float*, const R&, const R::Params&, bool, int, \
+                                      int, cudaStream_t, const uint32_t*);
+BAGUA_SHARD_UPDATE(SgdRule)
+BAGUA_SHARD_UPDATE(AdamRule)
+BAGUA_SHARD_UPDATE(LionRule)
+BAGUA_SHARD_UPDATE(LambRule)
+BAGUA_SHARD_UPDATE(LarsRule)
+#undef BAGUA_SHARD_UPDATE
+
 
 void launch_shard_publish(const PeerCtx& ctx, const PeerBuf& weights, size_t w_off, size_t bytes, int dtype, const float* src, bool use_multimem,
                           int nblocks, int nthreads, cudaStream_t stream) {

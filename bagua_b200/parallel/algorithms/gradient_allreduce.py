@@ -66,6 +66,10 @@ _HYPER = {"sgd": lambda g: (float(g["lr"]), float(g["momentum"]), float(g["dampe
 # the rules whose trust ratio is a norm over a whole parameter: phase A in the bucket program, then per-bucket norms, one
 # per-parameter exchange and the per-bucket update in step()
 _PER_PARAMETER = ("lamb", "lars")
+# the native ops of a rule: the fused bucket op (update inside backward; none for the per-parameter rules) and the phase-B op step() runs.
+# Both constructors take the rule's fp32 state in _STATE_KEYS order; the per-parameter rules' phase-B op is built by _per_param_ops.
+_OPS = {"sgd": ("AllReduceSgdOp", "ShardSgdOp"), "adam": ("AllReduceAdamOp", "ShardAdamOp"), "lion": ("AllReduceLionOp", "ShardLionOp"),
+        "lamb": (None, "ShardLambOp"), "lars": (None, "ShardLarsOp")}
 
 
 def consolidate_shards(shards, numel: int, layout):
@@ -624,19 +628,22 @@ def _check_bound(max_grad_norm):
     return None if max_grad_norm is None else float(max_grad_norm)
 
 
-def _set_ema(opt, ema_decay, ema_every):
+def _configure(opt, max_grad_norm, loss_scaling, accumulate_grads, ema_decay, ema_every):
+    """The options every sharded in-bucket optimizer factory takes."""
+    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
     if ema_decay is None:
-        return
+        return opt
     if not 0.0 < float(ema_decay) < 1.0:
         raise ValueError(f"ema_decay must be a number in (0, 1) or None, got {ema_decay}")
     if int(ema_every) != ema_every or int(ema_every) < 1:
         raise ValueError(f"ema_every must be a positive integer, got {ema_every}")
     opt._ema, opt.ema_decay, opt.ema_every = True, float(ema_decay), int(ema_every)
+    return opt
 
 
 def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, max_grad_norm=None, loss_scaling=False,
                            accumulate_grads=False, ema_decay=None, ema_every=1):
-    """SGD whose update runs *inside* each bucket's NVSwitch kernel (``allreduce_sgd_kernel``): reduce-scatter of the
+    """SGD whose update runs *inside* each bucket's NVSwitch kernel (``allreduce_update_kernel``): reduce-scatter of the
     gradients → SGD(momentum) on this rank's 1/N shard with fp32 master weights → all-gather of the updated weights, one
     launch per bucket, overlapped with the rest of backward.  Optimizer state is sharded N ways (ZeRO-1-like) and the
     gradient bucket is cleared on the way out.  Use together with ``FusedGradientAllReduceAlgorithm``; with one process (or
@@ -668,9 +675,7 @@ def make_sharded_fused_sgd(params, lr=1e-3, momentum=0.0, dampening=0.0, weight_
 
     opt = _ShardedFusedSGD(params, lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
                            master_weights=True, zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
-    _set_ema(opt, ema_decay, ema_every)
-    return opt
+    return _configure(opt, max_grad_norm, loss_scaling, accumulate_grads, ema_decay, ema_every)
 
 
 class ShardedFusedAdam(object):
@@ -680,7 +685,7 @@ class ShardedFusedAdam(object):
 def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, adamw=False, max_grad_norm=None, loss_scaling=False,
                             accumulate_grads=False, ema_decay=None, ema_every=1):
     """Adam / AdamW counterpart of :func:`make_sharded_fused_sgd`: the update of this rank's 1/N shard (fp32 master weights
-    and both moments) runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_adam_kernel``).  With one
+    and both moments) runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_update_kernel``).  With one
     process (or without a peer engine) it behaves like :class:`bagua_b200.ops.optim.FusedAdam`.  ``max_grad_norm``,
     ``loss_scaling``, ``accumulate_grads``: see :func:`make_sharded_fused_sgd`."""
     from ...ops.optim import FusedAdam
@@ -690,9 +695,7 @@ def make_sharded_fused_adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weigh
 
     opt = _ShardedFusedAdam(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, adamw=adamw, master_weights=True,
                             zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
-    _set_ema(opt, ema_decay, ema_every)
-    return opt
+    return _configure(opt, max_grad_norm, loss_scaling, accumulate_grads, ema_decay, ema_every)
 
 
 class ShardedFusedLamb(object):
@@ -720,9 +723,7 @@ def make_sharded_fused_lamb(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weigh
         _kind = "lamb"
 
     opt = _ShardedFusedLamb(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, master_weights=True, zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
-    _set_ema(opt, ema_decay, ema_every)
-    return opt
+    return _configure(opt, max_grad_norm, loss_scaling, accumulate_grads, ema_decay, ema_every)
 
 
 class ShardedFusedLars(object):
@@ -749,9 +750,7 @@ def make_sharded_fused_lars(params, lr=1e-3, momentum=0.9, weight_decay=0.0, tru
 
     opt = _ShardedFusedLars(params, lr=lr, momentum=momentum, weight_decay=weight_decay, trust_coefficient=trust_coefficient, master_weights=True,
                             zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
-    _set_ema(opt, ema_decay, ema_every)
-    return opt
+    return _configure(opt, max_grad_norm, loss_scaling, accumulate_grads, ema_decay, ema_every)
 
 
 class ShardedFusedLion(object):
@@ -762,9 +761,9 @@ def make_sharded_fused_lion(params, lr=1e-4, betas=(0.9, 0.99), weight_decay=0.0
                             ema_decay=None, ema_every=1):
     """Lion (see :class:`bagua_b200.ops.optim.FusedLion`) on the in-bucket sharded path: each rank keeps fp32 master weights and the
     one moment ``exp_avg`` for its 1/N slice of every bucket, 4 bytes per element / N less than Adam. The rule is element-wise, so
-    like SGD and Adam the update runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_lion_kernel``),
+    like SGD and Adam the update runs inside each bucket's reduce-scatter → all-gather kernel (``allreduce_update_kernel``),
     overlapped with the rest of backward. With ``max_grad_norm``, ``loss_scaling`` or ``accumulate_grads`` the bucket kernels only
-    reduce-scatter into the fp32 gradient shard and ``step()`` runs the update (``shard_lion_kernel``); see
+    reduce-scatter into the fp32 gradient shard and ``step()`` runs the update (``shard_update_kernel``); see
     :func:`make_sharded_fused_sgd`. With one process, or without a peer engine, it behaves like :class:`bagua_b200.ops.optim.FusedLion`."""
     from ...ops.optim import FusedLion
 
@@ -772,9 +771,7 @@ def make_sharded_fused_lion(params, lr=1e-4, betas=(0.9, 0.99), weight_decay=0.0
         _kind = "lion"
 
     opt = _ShardedFusedLion(params, lr=lr, betas=betas, weight_decay=weight_decay, master_weights=True, zero_grad_in_step=True)
-    opt.max_grad_norm, opt.loss_scaling, opt.accumulate_grads = _check_bound(max_grad_norm), bool(loss_scaling), bool(accumulate_grads)
-    _set_ema(opt, ema_decay, ema_every)
-    return opt
+    return _configure(opt, max_grad_norm, loss_scaling, accumulate_grads, ema_decay, ema_every)
 
 
 class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
@@ -882,13 +879,10 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         bucket.clear_ops()
         eng = bucket._engine(self.process_group)
         opt = self.optimizer
-        is_adam = isinstance(opt, ShardedFusedAdam)
-        is_lamb = isinstance(opt, ShardedFusedLamb)
-        is_lars = isinstance(opt, ShardedFusedLars)
-        is_lion = isinstance(opt, ShardedFusedLion)
-        per_param = is_lamb or is_lars
-        if eng is None or bucket._slice is None or not (isinstance(opt, ShardedFusedSGD) or is_adam or per_param or is_lion):
+        if eng is None or bucket._slice is None or not isinstance(opt, _ShardedStateMixin):
             return super().init_operations(bagua_ddp, bucket)
+        kind = opt._kind
+        per_param = kind in _PER_PARAMETER
         bk = opt._bucketing
         group_index = getattr(bucket, "_fused_group", 0)
         C = native()
@@ -920,7 +914,8 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         master = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
         if hi > lo:
             master[: hi - lo].copy_(wflat[lo:hi].float())
-        momentum = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device)
+        # the rule's fp32 state in _STATE_KEYS order: the master, then its moments
+        state = (master,) + tuple(torch.zeros(vpr * per, dtype=torch.float32, device=flat.device) for _ in _STATE_KEYS[kind][1:])
         # NVLS whenever the fabric offers it (the variant validated on 2 and 8 GPUs); peer ld/st two-shot otherwise
         use_mc = bool(wslice.has_multicast and bucket._slice.has_multicast and eng.has_multicast)
         # with 2 ranks the in-switch reduction buys nothing (each GPU pulls half the bucket either way), so the peer ld/st
@@ -933,14 +928,13 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
         cfg = eng.launch_cfg("multimem" if use_mc else "two_shot", nbytes, blocks=int(os.environ.get("BAGUA_FUSED_BLOCKS", "0")) or (16 if use_mc else 64))
         scale = (1.0 / n) if self.average else 1.0
         code = dtype_code(flat.dtype)
-        second = torch.zeros(vpr * per, dtype=torch.float32, device=flat.device) if is_adam or is_lamb else None
         clip, scaled, accum = opt.max_grad_norm is not None, opt.loss_scaling, opt.accumulate_grads
         exchange = clip or scaled   # the norm exchange runs in step(), so the update does too
         two_phase = exchange or per_param or accum
         layout = [(t.bagua_tensor_name, (t.bagua_getter_closure().data_ptr() - base) // flat.element_size(), t.bagua_getter_closure().numel(),
                    tuple(t.shape), tuple(dense_strides(t))) for t in bucket.tensors if not t.bagua_tensor_name.startswith("bagua_padding_tensor")]
         rec = {"bucket": bucket.name, "group": self.process_group, "numel": flat.numel(), "lo": lo, "hi": hi, "layout": layout,
-               "state": (master, momentum, second) if is_adam or is_lamb else (master, momentum), "weights": wflat,
+               "state": state, "weights": wflat,
                "param_ids": [id(t) for t in bucket.tensors], "shard": None}
         if opt._ema:
             # the EMA shard starts equal to the master (a carried-over or loaded state overwrites both); publishing it, or the master
@@ -968,33 +962,21 @@ class FusedGradientAllReduceAlgorithmImpl(GradientAllReduceAlgorithmImpl):
             bucket.backend_bucket.append_op(red)
             bucket._ops_keepalive.append(red)
             coef_ptr = bk.clip["out"][1:].data_ptr() if exchange else (bk.unit.data_ptr() if not per_param else 0)
+        fused_op, shard_op = _OPS[kind]
+        ptrs = [t.data_ptr() for t in state]
         if per_param:
-            op, moments = self._per_param_ops(eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr, is_lars)
-        elif two_phase and is_lion:
-            op = C.ShardLionOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
-                               use_mc, cfg)
-        elif two_phase and is_adam:
-            op = C.ShardAdamOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
-                               second.data_ptr(), use_mc, cfg)
+            op, moments = self._per_param_ops(eng, bk, rec, wslice, nbytes, code, use_mc, cfg, coef_ptr, kind == "lars")
         elif two_phase:
-            op = C.ShardSgdOp(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, master.data_ptr(), momentum.data_ptr(),
-                              use_mc, cfg)
-        elif is_lion:
-            op = C.AllReduceLionOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
-                                   master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
-        elif is_adam:
-            op = C.AllReduceAdamOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
-                                   master.data_ptr(), momentum.data_ptr(), second.data_ptr(), scale, True, use_mc, cfg)
+            op = getattr(C, shard_op)(eng.comm, wslice.buf, wslice.offset, nbytes, code, shard.data_ptr(), coef_ptr, *ptrs, use_mc, cfg)
         else:
-            op = C.AllReduceSgdOp(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code,
-                                  master.data_ptr(), momentum.data_ptr(), scale, True, use_mc, cfg)
+            op = getattr(C, fused_op)(eng.comm, bucket._slice.buf, wslice.buf, bucket._slice.offset, wslice.offset, nbytes, code, *ptrs, scale, True,
+                                      use_mc, cfg)
         if two_phase:
             bk.update_ops.append(op)
         else:
             bucket.backend_bucket.append_op(op)
         bucket._ops_keepalive.append(op)
-        kind = "fused_lamb_" if is_lamb else ("fused_lars_" if is_lars else ("fused_lion_" if is_lion else ("fused_adam_" if is_adam else "fused_sgd_")))
-        bucket.allreduce_variant = kind + ("accum_" if accum else "") + ("scaled_" if scaled else "") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
+        bucket.allreduce_variant = f"fused_{kind}_" + ("accum_" if accum else "") + ("scaled_" if scaled else "") + ("clip_" if clip else "") + ("multimem" if use_mc else "two_shot")
         rec["step_ops"] = (op, moments) if per_param else (op,)   # the update op first: state_dict() saves its count
         if scaled:   # the ops obey the exchange's vote and take the step count it keeps on the device
             for o in rec["step_ops"]:

@@ -77,11 +77,11 @@ sgd = C.AllReduceSgdOp(comm, a.buf, b.buf, 0, 0, NB, code, master.data_ptr(), mo
 sgd.set_hyper(0.01, 0.9, 0.0, 1e-4, False)
 run(sgd)  # first step initialises the momentum
 # reads grads (2B) + master, momentum (8B); writes master, momentum (8B) + weights (2B) + zeroed grads (2B) per element
-timed("allreduce_sgd_kernel<bf16,P=1,peer> 64MiB bucket, momentum", lambda: run(sgd), n * 22)
+timed("allreduce_update_kernel<bf16,P=1,peer,SgdRule> 64MiB bucket, momentum", lambda: run(sgd), n * 22)
 m2 = torch.zeros(n, device=dev)
 adam = C.AllReduceAdamOp(comm, a.buf, b.buf, 0, 0, NB, code, master.data_ptr(), mom.data_ptr(), m2.data_ptr(), 1.0, True, False, w.cfg(32))
 adam.set_hyper(1e-3, 0.9, 0.999, 1e-8, 0.01, True)
-timed("allreduce_adam_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(adam), n * 30)
+timed("allreduce_update_kernel<bf16,P=1,peer,AdamRule> 64MiB bucket", lambda: run(adam), n * 30)
 rs = C.ReduceScatterOp(comm, a.buf, 0, NB, code, 1.0, False, w.cfg(32))
 timed("reduce_scatter_kernel<bf16,P=1> 64MiB", lambda: run(rs), 2 * NB)
 ag = C.AllGatherOp(comm, a.buf, 0, NB, code, False, w.cfg(32))
@@ -127,7 +127,7 @@ lsegs = torch.tensor([0, n, 0], dtype=torch.int32, device=dev)
 lapply = C.ShardLambOp(comm, b.buf, 0, NB, code, master.data_ptr(), mom.data_ptr(), m2.data_ptr(), lsegs.data_ptr(), 1, lratio.data_ptr(), False, w.cfg(32))
 lapply.set_hyper(1e-3, 0.9, 0.999, 1e-6, 0.01)
 # reads master and both moments (12B); writes master (4B) + weights (2B) per element
-timed("shard_lamb_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(lapply), n * 18)
+timed("shard_update_kernel<bf16,P=1,peer,LambRule> 64MiB bucket", lambda: run(lapply), n * 18)
 # in-bucket LARS on the same bucket as ONE parameter: stage-1 norms over [master, shard], apply from the exchanged sums
 nplan = multi_tensor_plan([[master], [shard]])
 npart = torch.zeros(nplan.n_blocks, 2, dtype=torch.float64, device=dev)
@@ -138,7 +138,7 @@ lsums.copy_(torch.tensor([[float(n), float(n)]], dtype=torch.float64))
 lars = C.ShardLarsOp(comm, b.buf, 0, NB, code, shard.data_ptr(), 0, master.data_ptr(), mom.data_ptr(), lsegs.data_ptr(), 1, lsums.data_ptr(), False, w.cfg(32))
 lars.set_hyper(1e-3, 0.9, 5e-4, 1e-3)
 # reads shard, master, momentum (12B); writes master, momentum (8B) + weights (2B) per element
-timed("shard_lars_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(lars), n * 22)
+timed("shard_update_kernel<bf16,P=1,peer,LarsRule> 64MiB bucket", lambda: run(lars), n * 22)
 # phase A into the same shard: overwrite (reads the bucket 2B, writes the shard 4B) and accumulate (+ reads the shard 4B) per element
 gpart = torch.zeros(C.MAX_COMM_BLOCKS, dtype=torch.float64, device=dev)
 for acc, nb in ((False, 6), (True, 10)):
@@ -157,11 +157,11 @@ timed("shard_publish_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(pub), n * 
 # weights 2B and the cleared bucket 2B per element) and phase B (reads shard, master, exp_avg 12B; writes 8B + the weights 2B)
 lion = C.AllReduceLionOp(comm, a.buf, b.buf, 0, 0, NB, code, master.data_ptr(), mom.data_ptr(), 1.0, True, False, w.cfg(32))
 lion.set_hyper(1e-4, 0.9, 0.99, 0.1)
-timed("allreduce_lion_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(lion), n * 22)
+timed("allreduce_update_kernel<bf16,P=1,peer,LionRule> 64MiB bucket", lambda: run(lion), n * 22)
 unit = torch.ones(1, device=dev)
 slion = C.ShardLionOp(comm, b.buf, 0, NB, code, shard.data_ptr(), unit.data_ptr(), master.data_ptr(), mom.data_ptr(), False, w.cfg(64))
 slion.set_hyper(1e-4, 0.9, 0.99, 0.1)
-timed("shard_lion_kernel<bf16,P=1,peer> 64MiB bucket", lambda: run(slion), n * 22)
+timed("shard_update_kernel<bf16,P=1,peer,LionRule> 64MiB bucket", lambda: run(slion), n * 22)
 del shard, lpart, npart, gpart, eshard
 
 # single-GPU kernels ------------------------------------------------------------------------------------------------------

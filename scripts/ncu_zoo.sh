@@ -12,7 +12,7 @@ ncu -i /tmp/ncu_zoo.ncu-rep --page details --csv > "$out/ncu_zoo_details.csv" 2>
 sz=$(stat -c %s /tmp/ncu_zoo.ncu-rep 2>/dev/null || echo 0)
 if [ "$sz" -lt 30000000 ] && [ "$sz" -gt 0 ]; then cp /tmp/ncu_zoo.ncu-rep "$out/"; fi
 # source-level capture (SASS + source lines, stall reasons) of the three headline kernels only
-for k in allreduce_sgd_kernel bytegrad_kernel grouped_gemm_tn_kernel; do
+for k in allreduce_update_kernel bytegrad_kernel grouped_gemm_tn_kernel; do
   ZOO_NCU=1 timeout 600 ncu --set full --clock-control none --import-source on -k "regex:$k" -c 1 -o /tmp/ncu_$k -f python scripts/kernel_zoo.py >> "$out/ncu_zoo.log" 2>&1
   ncu -i /tmp/ncu_$k.ncu-rep --page source --csv > "$out/ncu_${k}_source.csv" 2>> "$out/ncu_zoo.log"
   s2=$(stat -c %s /tmp/ncu_$k.ncu-rep 2>/dev/null || echo 0)

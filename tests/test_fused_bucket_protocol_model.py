@@ -1,4 +1,4 @@
-"""Schedule-exploring model of ``allreduce_sgd_kernel`` / ``allreduce_adam_kernel`` (bagua_b200/csrc/peer_kernels.cu): one launch per
+"""Schedule-exploring model of ``allreduce_update_kernel`` (bagua_b200/csrc/peer_kernels.cu): one launch per
 bucket does  barrier → reduce-scatter (rank r pulls slice r of every peer's gradient bucket) → optimizer step on the slice →
 all-gather (pushes the new weights of slice r into every peer's weight bucket) → barrier → zero the own gradient bucket.
 
